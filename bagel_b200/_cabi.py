@@ -69,7 +69,7 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not LIB_PATH.exists():
             raise BagelB200Error(
-                f"{LIB_PATH} not found. Build it with `python -m bagel_b200.build` (needs nvcc, sm_100a). "
+                f"{LIB_PATH} not found. Build it with `python -m bagel_b200.build` (needs nvcc, sm_90a). "
                 "bagel_b200 has no CPU or PyTorch fallback.")
         l = C.CDLL(str(LIB_PATH))
         for name, (res, args) in SIGNATURES.items():

@@ -3,8 +3,8 @@
 Same surface as the reference: `AutoEncoderParams`, `AutoEncoder(params).encode(x) / .decode(z)`, `load_ae(path)`
 returning `(ae, params)`; state-dict keys follow the reference's module names (SURVEY.md §8b).
 
-Execution model (B200-first): activations are NHWC bf16 and stay on the device; every convolution is the
-implicit-GEMM tcgen05 kernel (bagel_conv2d_nhwc_bf16: no im2col buffer, the 3x3 taps are K-slices fetched by 4-D
+Execution model (GPU-first): activations are NHWC bf16 and stay on the device; every convolution is the
+implicit-GEMM wgmma kernel (bagel_conv2d_nhwc_bf16: no im2col buffer, the 3x3 taps are K-slices fetched by 4-D
 TMA boxes whose out-of-image coordinates are the zero padding, stride-2 via TMA element strides, bias and the
 ResnetBlock skip connection fused in the epilogue); GroupNorm(32)+swish is a deterministic two-stage reduction +
 one fused normalise/activate pass; 1x1 convs of the attention block are plain GEMMs; the single-head d=512

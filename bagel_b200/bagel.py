@@ -1,11 +1,11 @@
-"""BAGEL unified model — host side of the B200-native build.
+"""BAGEL unified model — host side of the H100-native build.
 
 Same public surface as the reference's modeling/bagel/bagel.py (Bagel :57): the `prepare_*` packers
 (:232-264, :552-641, :909-927) return dicts with the same keys / dtypes (key names are API — callers splat
 them as kwargs), `forward_cache_update_text` (:267-297) prefill, the rectified-flow sampler `generate_image`
 (:644-754) with `_forward_flow` (:757-907), and `generate_text` (:930-1000).
 
-What is different underneath (B200-first, not a port):
+What is different underneath (GPU-first, not a port):
   * packers are vectorised index arithmetic (no per-token Python loops);
   * `generate_image` plans the whole run once (index maps, RoPE tables, all timestep embeddings, merged KV
     buffers with the read-only context already in place), batches the CFG branches into ONE packed LM call per
@@ -579,7 +579,7 @@ class Bagel:
         token ids on the model's device. As in the reference, generation stops when SAMPLE 0 emits `end_token_id`
         (:996) and the stopping token is not returned.
 
-        B200-first execution (the reference re-allocates and re-scatters the whole KV cache per layer per token and
+        GPU-first execution (the reference re-allocates and re-scatters the whole KV cache per layer per token and
         rebuilds index tensors with host loops): the KV cache is copied ONCE into per-sample slabs with room for
         `max_length` new tokens; sequence lengths, RoPE positions, write slots and the token history live on the
         device; a step is embedding gather -> 28 layers (fused QKV epilogue appends K/V in place, attention reads
@@ -602,7 +602,7 @@ class Bagel:
         max_kv = int(cap.max())   # host upper bound of any sample's key count (sizes the key split of decode attention)
         has_ctx = past_key_values is not None and past_key_values.key_cache[0] is not None and int(kv.sum()) > 0
         # zero-filled, not torch.empty: attention multiplies the masked probabilities (exactly 0) with whatever sits in the
-        # spare rows of a slab — 0 x NaN/Inf garbage would poison the output (the tcgen05 kernel fetches whole 128-key
+        # spare rows of a slab — 0 x NaN/Inf garbage would poison the output (the attention kernel fetches whole 128-key
         # blocks by TMA; only the single-query d=128 kernel clamps its loads to the rows in use)
         kbuf = torch.zeros((L, total, w), dtype=BF16, device=dev)
         vbuf = torch.zeros((L, total, w), dtype=BF16, device=dev)
@@ -710,7 +710,7 @@ class Bagel:
                 packed_vit_token_indexes=None, packed_vit_position_ids=None, vit_token_seqlens=None, padded_latent=None,
                 patchified_vae_latent_shapes=None, packed_latent_position_ids=None, packed_vae_token_indexes=None,
                 packed_timesteps=None, mse_loss_indexes=None, noise: Optional[torch.Tensor] = None):
-        """The reference's training forward on a packed batch -> dict(mse=..., ce=...) (forward only: the B200 build has no
+        """The reference's training forward on a packed batch -> dict(mse=..., ce=...) (forward only: this build has no
         autograd; useful for evaluation losses / distillation targets with the inference kernels).
 
         Attention structure (data/data_utils.py:13-40, 72-103): every sample is a list of splits that are 'causal' (text),

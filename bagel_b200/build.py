@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (bagel_b200/libbagel_b200.so) in-tree with nvcc for sm_100a.
+"""Build the C-ABI shared library (bagel_b200/libbagel_b200.so) in-tree with nvcc for sm_90a (H100).
 
 No JIT cache, no torch.utils.cpp_extension: the library has no torch types in its interface, so it is a
 plain `nvcc -shared`. The built .so is git-ignored but travels with the tree to the GPU box.
@@ -18,7 +18,7 @@ LIB_PATH = PKG_DIR / "libbagel_b200.so"
 STAMP = PKG_DIR / ".libbagel_b200.stamp"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -28,7 +28,7 @@ NVCC_FLAGS = [
 def _nvcc() -> str:
     cand = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(cand):
-        raise RuntimeError("nvcc not found; bagel_b200 needs the CUDA toolkit to build its sm_100a kernels")
+        raise RuntimeError("nvcc not found; bagel_b200 needs the CUDA toolkit to build its sm_90a kernels")
     return cand
 
 
@@ -77,7 +77,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if failed:
         raise RuntimeError("bagel_b200: CUDA build failed")
     tmp = objdir / (LIB_PATH.name + ".tmp")   # link beside the objects, then rename: a reader never sees a partial library
-    link = [nvcc, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a"]
+    link = [nvcc, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"bagel_b200: link failed:\n{r.stdout}")

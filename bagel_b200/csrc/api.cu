@@ -46,10 +46,10 @@ bool pdl_small_enabled() {
   return on;
 }
 
-int require_sm100() {
+int require_sm90() {
   const DevInfo& d = dev_info();
-  if (d.major != 10)
-    return set_error(BAGEL_ERR_ARCH, "bagel_b200 kernels are sm_100a only; current device is sm_%d*", d.major * 10);
+  if (d.major != 9)
+    return set_error(BAGEL_ERR_ARCH, "bagel_b200 kernels are sm_90a only; current device is sm_%d*", d.major * 10);
   return 0;
 }
 

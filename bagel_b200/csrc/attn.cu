@@ -1,22 +1,16 @@
-// Packed variable-length flash attention forward for sm_100a (tcgen05 + TMEM + TMA).
+// Packed variable-length flash attention forward for sm_90a (wgmma + TMA + mbarrier).
 //
 // Drop-in for the reference's only native seam, flash_attn_varlen_func (FA2, mma.sync) as called at
 // modeling/bagel/qwen2_navit.py:361-370, 579-588 and modeling/bagel/siglip_navit.py:232-241:
 //   out[Sq,Hq,D] = softmax(q k^T * scale [+ bottom-right causal mask]) v   per packed sample, GQA by Hq % Hk == 0,
 //   bf16 in / fp32 softmax + accumulation / bf16 out.
 //
-// PERSISTENT kernel, one CTA per SM. A work item = TWO 128-row query tiles of one (sample, head), swept over that sample's
-// keys in blocks of 128; items are handed out by a device-side counter (dynamic scheduling):
-//   warps 0-3 / 4-7   softmax group of tile 0 / tile 1: tcgen05.ld S -> online softmax -> P (bf16) back into the S columns of
-//                     TMEM; rescales O in TMEM when the running max jumps; final O / l -> global
-//   warp 8            scheduler + TMA producer: fetches the next item (atomicAdd, published through shared memory), loads its
-//                     Q tiles (as soon as the previous item's last QK^T has read Q), then K_j / V_j through a smem ring
-//   warp 9            MMA issuer (one lane): S_t = Q_t K_j^T  (SS, both K-major)  and  O_t += P_t V_j (TS: A = P in TMEM,
-//                     B = V MN-major) — the tensor pipe runs tile 0 while tile 1 is in softmax and vice versa; the first
-//                     QK^T of the next item is issued while the softmax warps still write out the current item's O
-// TMEM map (512 columns): S0 [0,128) S1 [128,256) O0 [256,256+D) O1 [384,384+D); P_t aliases S_t columns [0,64).
-// (Round 1's one-CTA-per-item grid paid launch + TMEM allocation + barrier set-up + pipeline ramp per item: ~4 key blocks
-// worth of time, i.e. 33 % at L = 1k. Its "two threads per score row" variant was measured slower and is gone.)
+// One CTA per 128-row query tile of one (sample, head), swept over that sample's keys in blocks of 128:
+//   warp 8           TMA producer (one elected lane): the Q tile, then K_j / V_j through a smem ring
+//   warpgroups 0, 1  64 query rows each: S = Q K_j^T (wgmma, both K-major, fp32 in registers) -> online softmax in
+//                    registers -> P (bf16) stays in registers as the A operand of O += P V_j (wgmma, V MN-major)
+// The two MMA warpgroups run out of phase on their own: one is in its softmax while the other's wgmmas occupy the tensor
+// cores.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -24,31 +18,15 @@
 #include <stdio.h>
 #include <stdlib.h>
 
-#include <atomic>
-#include <type_traits>
-
 #include "common.cuh"
 #include "host_util.h"
 #include "attn_decode.h"
-#include "attn3.h"
 
 namespace bagel {
 
-// Optional timeline instrumentation (tools/gpu_attn_trace.py builds a separate library with -DBAGEL_ATTN_TRACE; the product
-// library never defines it): CTA 0 records clock64() stamps of the softmax warps 0 / 4 and the MMA lane for its first blocks.
-#ifdef BAGEL_ATTN_TRACE
-constexpr int kTraceIters = 1024, kTraceEvents = 8;
-__device__ long long g_attn_trace[3 * kTraceIters * kTraceEvents];
-#define ATTN_TRACE(role, iter, ev)                                                                   \
-  do {                                                                                               \
-    if (blockIdx.x == 0 && (iter) < kTraceIters) g_attn_trace[((role) * kTraceIters + (iter)) * kTraceEvents + (ev)] = clock64(); \
-  } while (0)
-#else
-#define ATTN_TRACE(role, iter, ev) do { } while (0)
-#endif
-
-constexpr int kAttnThreads = (8 + 2) * 32;  // softmax warps of both tiles (4 + 4) + TMA warp + MMA warp
-constexpr int kBlockM = 128;  // rows per query tile (2 tiles per work item)
+constexpr int kAttnThreads = 2 * 128 + 32;   // two MMA warpgroups + the producer warp (<= 224 registers per thread)
+constexpr int kAttnMmaWarps = 8;
+constexpr int kBlockM = 128;  // query rows per CTA (64 per MMA warpgroup)
 constexpr int kBlockN = 128;  // keys per block
 
 struct AttnParams {
@@ -60,39 +38,15 @@ struct AttnParams {
   int Hq, Hk;
   int causal;
   float scale_log2;  // softmax_scale * log2(e)
-  int qtiles;        // work items per (sample, head): ceil(max_seqlen_q / 256)
-  int num_items;     // qtiles * Hq * batch
-  int* sched;        // device counter (zeroed before the launch): next work item to hand out
-  int poly;          // every 4th score pair of interior key blocks takes the FMA-pipe exp2 (BAGEL_ATTN_POLY)
+  int poly;          // every 4th score pair of unmasked key blocks takes the FMA-pipe exp2 (BAGEL_ATTN_POLY)
 };
 
 template <int D>
 struct AttnCfg {
-  static constexpr int kTileBytes = kBlockM * D * 2;  // one Q tile / one K block / one V block
-// 4 stages measured equal or better than 5 on one box (profiles/r02_attn_poly_stages_ab.txt); -D for A/B builds
-#ifndef BAGEL_ATTN_STAGES128
-#define BAGEL_ATTN_STAGES128 4
-#endif
-  static constexpr int kStages = (D == 128) ? BAGEL_ATTN_STAGES128 : 6;
-  static constexpr int kSmemBytes = 2 * kTileBytes + kStages * kTileBytes + 1024 + 512;
+  static constexpr int kTileBytes = kBlockM * D * 2;  // the Q tile / one K block / one V block
+  static constexpr int kStages = (D == 128) ? 4 : 6;
+  static constexpr int kSmemBytes = kTileBytes + kStages * kTileBytes + 1024 + 256;
 };
-
-// packed fp32x2 arithmetic (sm_100): one issue slot for two lanes of FMA / ADD
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)),
-        "l"(*reinterpret_cast<unsigned long long*>(&c)));
-  return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  unsigned long long d;
-  asm("add.rn.f32x2 %0, %1, %2;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&d);
-}
 
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -102,116 +56,28 @@ __device__ __forceinline__ float ex2(float x) {
 
 // 2^x on the FMA pipe for a PAIR of scores (no MUFU): round-to-nearest split x = n + f through the 1.5 * 2^23 magic add,
 // degree-3 minimax polynomial of 2^f on [-0.5, 0.5] (max relative error 1.0e-4, 40x below the bf16 rounding of P), and n added
-// to the exponent field with one integer multiply-add. Valid for x <= ~100; x below -126 (masked-out -inf included) clamps to
-// 2^-126, NOT to 0 — so it is only used in interior key blocks, never where a mask could leave a row without any visible key.
-// With one softmax warp of each tile per SM sub-partition the exp2 stream is MUFU-bound (16 exp2 / clk / SM = 2048 clk per
-// pair of 128 x 128 blocks, as long as the two tensor-core GEMMs of those blocks); every 4th score pair goes through this path.
+// to the exponent field with one integer add. Valid for x <= ~100; x below -126 (masked-out -inf included) clamps to
+// 2^-126, NOT to 0 — so it is only used in unmasked key blocks. The MUFU unit (16 exp2 / clk / SM) is the softmax's
+// bottleneck; every 4th score pair goes through this path instead.
 __device__ __forceinline__ float2 ex2_poly2(float2 x) {
-  const float2 magic = make_float2(12582912.0f, 12582912.0f), neg_magic = make_float2(-12582912.0f, -12582912.0f);
-  const float2 neg1 = make_float2(-1.0f, -1.0f), one = make_float2(1.0f, 1.0f);
+  const float2 magic = make_float2(12582912.0f, 12582912.0f);
   const float2 c1 = make_float2(0.69328292f, 0.69328292f), c2 = make_float2(0.24221068f, 0.24221068f),
                c3 = make_float2(0.05500873f, 0.05500873f);
   x.x = fmaxf(x.x, -126.0f);
   x.y = fmaxf(x.y, -126.0f);
-  const float2 t = fadd2(x, magic);            // integer part in the low mantissa bits
-  const float2 n = fadd2(t, neg_magic);        // exact
-  const float2 f = ffma2(n, neg1, x);          // x - n, in [-0.5, 0.5]
-  float2 q = ffma2(f, c3, c2);
-  q = ffma2(q, f, c1);
-  q = ffma2(q, f, one);
+  const float2 t = make_float2(x.x + magic.x, x.y + magic.y);     // integer part in the low mantissa bits
+  const float2 n = make_float2(t.x - magic.x, t.y - magic.y);     // exact
+  const float2 f = make_float2(x.x - n.x, x.y - n.y);             // in [-0.5, 0.5]
+  float2 q = make_float2(fmaf(f.x, c3.x, c2.x), fmaf(f.y, c3.y, c2.y));
+  q = make_float2(fmaf(q.x, f.x, c1.x), fmaf(q.y, f.y, c1.y));
+  q = make_float2(fmaf(q.x, f.x, 1.0f), fmaf(q.y, f.y, 1.0f));
   float2 r;
   r.x = __int_as_float(__float_as_int(q.x) + (__float_as_int(t.x) << 23));
   r.y = __int_as_float(__float_as_int(q.y) + (__float_as_int(t.y) << 23));
   return r;
 }
 
-// tcgen05.mma with the operand descriptors given by their LOW words only. All operand tiles of this kernel share the high
-// word (SBO = 1024 B, descriptor version 1, SWIZZLE_128B), and between the MMAs of one key block only the 14-bit start
-// address field (address >> 4) in the low word moves. The single issuing lane's instruction stream paces the whole loop
-// (ncu source view: ~80 cycles of ALU + ELECT + R2UR.BROADCAST + BRA.U.ANY per MMA against 58-64 cycles of tensor work), so
-// every 64-bit add-with-carry and every R2UR of a constant removed from it shortens the key-block period.
-constexpr uint32_t kDescHiSw128 = 0x40004040u;   // bits 32..63 of umma_desc_{kmajor,mnmajor}_sw128()
-__device__ __forceinline__ uint32_t desc_lo_kmajor(uint32_t smem_addr) { return (smem_addr & 0x3FFFF) >> 4; }
-__device__ __forceinline__ uint32_t desc_lo_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr & 0x3FFFF) >> 4) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
-}
-__device__ __forceinline__ void umma_ss_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b32 hi;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b32 hi, %5;\n\t"
-      "mov.b64 da, {%1, hi};\n\t"
-      "mov.b64 db, {%2, hi};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "n"(kDescHiSw128)
-      : "memory");
-}
-__device__ __forceinline__ void umma_ts_lo(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b32 hi;\n\t"
-      ".reg .b64 db;\n\t"
-      "mov.b32 hi, %5;\n\t"
-      "mov.b64 db, {%2, hi};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "r"(b_lo), "r"(idesc), "r"(accumulate), "n"(kDescHiSw128)
-      : "memory");
-}
-
-// One unit of work: two 128-row query tiles of one (sample, head) against that sample's keys.
-struct AttnItem {
-  int b, h, hk;
-  int q_beg, Lq, k_beg, Lk;
-  int q0;            // first query row (within the sample)
-  int shift;         // bottom-right aligned causal: key kv visible to query qi iff kv <= qi + shift
-  int nblk;          // key blocks to load (= the larger of the two tiles' counts)
-  int nblk_t[2];     // key blocks each tile sweeps: under a causal mask tile 0 stops one block before tile 1
-  bool valid;        // q0 < Lq
-  bool tile1_active;
-};
-
-__device__ __forceinline__ AttnItem attn_decode_item(int item, const AttnParams& p) {
-  AttnItem w;
-  // q tiles of one (sample, head) are consecutive items: the CTAs running at any moment share those K/V blocks through the
-  // L2. Causal: the LAST query tiles sweep the most keys — hand them out first (longest-processing-time-first).
-  const int qi = item % p.qtiles;
-  const int bh = item / p.qtiles;
-  w.h = bh % p.Hq;
-  w.b = bh / p.Hq;
-  w.hk = w.h / (p.Hq / p.Hk);
-  const int qt = p.causal ? (p.qtiles - 1 - qi) : qi;
-  w.q_beg = p.cu_q[w.b];
-  w.Lq = p.cu_q[w.b + 1] - w.q_beg;
-  w.k_beg = p.cu_k[w.b];
-  w.Lk = p.seqused_k ? p.seqused_k[w.b] : (p.cu_k[w.b + 1] - w.k_beg);
-  w.q0 = qt * 2 * kBlockM;
-  w.valid = w.q0 < w.Lq;
-  w.tile1_active = (w.q0 + kBlockM) < w.Lq;
-  w.shift = w.Lk - w.Lq;
-  w.nblk_t[0] = w.nblk_t[1] = 0;
-  for (int t = 0; t < 2; ++t) {
-    if (!w.valid || (t == 1 && !w.tile1_active)) continue;
-    int kv_end = w.Lk;
-    if (p.causal) {   // last key any row of this tile may see
-      const int q_hi = min(w.Lq, w.q0 + (t + 1) * kBlockM) - 1;
-      kv_end = max(0, min(w.Lk, q_hi + w.shift + 1));
-    }
-    w.nblk_t[t] = (kv_end + kBlockN - 1) / kBlockN;
-  }
-  w.nblk = max(w.nblk_t[0], w.nblk_t[1]);   // causal: tile 1 sees at least as many keys as tile 0
-  return w;
-}
-
-// PERSISTENT kernel: one CTA per SM loops over work items handed out by a device-side counter (dynamic scheduling: ragged
-// and causal batches balance themselves; launch, TMEM allocation, barrier set-up and the pipeline ramp are paid once per
-// SM instead of once per item, and the Q load / first QK^T of the next item overlap the epilogue of the current one).
+// grid (query tiles, Hq, batch)
 template <int D>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_varlen_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -221,443 +87,196 @@ attn_varlen_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   constexpr int kTileBytes = Cfg::kTileBytes;
   constexpr int kAtoms = D / 64;               // 64-column (128 B) swizzle atoms per row
   constexpr int kAtomBytes = kBlockM * 128;    // one [128 rows x 64 cols] box
-  constexpr int kSoftWarps = 4;                // softmax warps per tile
-  constexpr int kTmaWarp = 2 * kSoftWarps, kMmaWarp = 2 * kSoftWarps + 1;
+
+  // causal: the LAST query tiles sweep the most keys — start them first
+  const int qt = p.causal ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int q_beg = p.cu_q[b];
+  const int Lq = p.cu_q[b + 1] - q_beg;
+  const int q0 = qt * kBlockM;
+  if (q0 >= Lq) return;   // uniform over the CTA
+  const int hk = h / (p.Hq / p.Hk);
+  const int k_beg = p.cu_k[b];
+  const int Lk = p.seqused_k ? p.seqused_k[b] : (p.cu_k[b + 1] - k_beg);
+  const int shift = Lk - Lq;   // bottom-right aligned causal: key kv visible to query qi iff kv <= qi + shift
+  int kv_end = Lk;
+  if (p.causal) kv_end = max(0, min(Lk, min(Lq, q0 + kBlockM) - 1 + shift + 1));
+  const int nblk = (kv_end + kBlockN - 1) / kBlockN;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_q = smem;                      // 2 tiles
-  uint8_t* smem_kv = smem + 2 * kTileBytes;    // ring
+  uint8_t* smem_q = smem;
+  uint8_t* smem_kv = smem + kTileBytes;    // ring: K_0, V_0, K_1, V_1, ...
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_kv + kStages * kTileBytes);
-  uint64_t* q_full = bars;                 // [1]  TMA -> MMA: Q tiles of the item landed
-  uint64_t* q_empty = bars + 1;            // [1]  MMA -> TMA: last QK^T of the item has read Q
-  uint64_t* kv_full = bars + 2;            // [kStages]
-  uint64_t* kv_empty = kv_full + kStages;  // [kStages]
-  uint64_t* s_bar = kv_empty + kStages;    // [2]  MMA -> softmax: S_t(j) ready
-  uint64_t* p_bar = s_bar + 2;             // [2]  softmax -> MMA: P_t(j) written (and O_t rescaled)
-  uint64_t* o_bar = p_bar + 2;             // [2]  MMA -> softmax: final O_t of the item ready
-  uint64_t* o_free = o_bar + 2;            // [2]  softmax -> MMA: O_t read out, the next item may overwrite it
-  uint64_t* sched_full = o_free + 2;       // [2]  TMA warp -> everyone: next work item published
-  uint64_t* sched_empty = sched_full + 2;  // [2]  everyone -> TMA warp: slot consumed
-  volatile int* sched_item = reinterpret_cast<volatile int*>(sched_empty + 2);   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(const_cast<int*>(sched_item) + 2);
+  uint64_t* q_full = bars;                 // [1]
+  uint64_t* kv_full = bars + 1;            // [kStages]
+  uint64_t* kv_empty = kv_full + kStages;  // [kStages]  one arrive per MMA warp
 
+  const int wg = threadIdx.x >> 7;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == kTmaWarp && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
-    mbar_init(q_empty, 1);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&s_bar[t], 1);
-      mbar_init(&p_bar[t], kSoftWarps);
-      mbar_init(&o_bar[t], 1);
-      mbar_init(&o_free[t], kSoftWarps);
-      mbar_init(&sched_full[t], 1);
-      mbar_init(&sched_empty[t], 1 + 2 * kSoftWarps);   // MMA lane + one lane of every softmax warp
+      mbar_init(&kv_empty[i], kAttnMmaWarps);
     }
     fence_mbar_init();
   }
-  if (warp == kMmaWarp) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S[2] = {tmem_base + 0, tmem_base + 128};
-  const uint32_t tmem_O[2] = {tmem_base + 256, tmem_base + 384};
 
-  if (warp == kTmaWarp) {
-    // =========================== scheduler + TMA producer ===========================
-    if (elect_one_lane()) {
+  if (wg == 2) {
+    // =========================== TMA producer ===========================
+    if (elect_one_lane() && nblk > 0) {
+      mbar_expect_tx(q_full, kTileBytes);
+      for (int a = 0; a < kAtoms; ++a)
+        tma_load_2d(smem_q + a * kAtomBytes, &tmQ, q_full, h * D + a * 64, q_beg + q0, kEvictFirst);
       int stage = 0;
       uint32_t phase = 0;
-      uint32_t q_phase = 0;
-      int slot = 0;
-      uint32_t sphase = 0;
-      int next = atomicAdd(p.sched, 1);
-      while (true) {
-        const int item = next;
-        mbar_wait(&sched_empty[slot], sphase ^ 1);
-        sched_item[slot] = item;
-        mbar_arrive(&sched_full[slot]);
-        if (++slot == 2) { slot = 0; sphase ^= 1; }
-        if (item >= p.num_items) break;
-        next = atomicAdd(p.sched, 1);   // in flight while this item's loads are issued
-        const AttnItem w = attn_decode_item(item, p);
-        if (w.nblk == 0) continue;
-        const int ntile = w.tile1_active ? 2 : 1;
-        mbar_wait(q_empty, q_phase ^ 1);   // the previous item's last QK^T has read its Q tiles
-        q_phase ^= 1;
-        mbar_expect_tx(q_full, ntile * kTileBytes);
-        for (int t = 0; t < ntile; ++t)
+      for (int j = 0; j < nblk; ++j) {
+        for (int kv = 0; kv < 2; ++kv) {  // K_j then V_j
+          mbar_wait(&kv_empty[stage], phase ^ 1);
+          mbar_expect_tx(&kv_full[stage], kTileBytes);
+          const CUtensorMap* tm = kv == 0 ? &tmK : &tmV;
           for (int a = 0; a < kAtoms; ++a)
-            tma_load_2d(smem_q + t * kTileBytes + a * kAtomBytes, &tmQ, q_full, w.h * D + a * 64,
-                        w.q_beg + w.q0 + t * kBlockM, kEvictFirst);
-        for (int j = 0; j < w.nblk; ++j) {
-          for (int kv = 0; kv < 2; ++kv) {  // K_j then V_j
-            mbar_wait(&kv_empty[stage], phase ^ 1);
-            mbar_expect_tx(&kv_full[stage], kTileBytes);
-            const CUtensorMap* tm = kv == 0 ? &tmK : &tmV;
-            for (int a = 0; a < kAtoms; ++a)
-              tma_load_2d(smem_kv + stage * kTileBytes + a * kAtomBytes, tm, &kv_full[stage], w.hk * D + a * 64,
-                          w.k_beg + j * kBlockN, kEvictLast);
-            if (++stage == kStages) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // =========================== MMA issuer ===========================
-    if (elect_one_lane()) {
-      constexpr uint32_t idesc_qk = umma_idesc_bf16(kBlockM, kBlockN, 0, 0);  // S[128,128] = Q[128,D] K[128,D]^T
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(kBlockM, D, 0, 1);        // O[128,D] += P[128,128] V[128,D]
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t q_phase = 0;
-      uint32_t pcnt[2] = {0, 0};    // P blocks consumed per tile (parity of p_bar)
-      uint32_t icnt[2] = {0, 0};    // items processed per tile (parity of o_free)
-      int slot = 0;
-      uint32_t sphase = 0;
-      [[maybe_unused]] int tr_it = 0;
-
-      const uint32_t q_lo[2] = {desc_lo_kmajor(smem_u32(smem_q)), desc_lo_kmajor(smem_u32(smem_q + kTileBytes))};
-      auto issue_qk = [&](int t, int kstage) {
-        // K-major operands: D columns = kAtoms atoms of 64 (+1024 in the address field per 16 KB atom); 4 UMMA_K=16 steps per
-        // atom (+2 = 32 B each)
-        const uint32_t k_lo = desc_lo_kmajor(smem_u32(smem_kv + kstage * kTileBytes));
-#pragma unroll
-        for (int a = 0; a < kAtoms; ++a) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint32_t off = (uint32_t)(a * (kAtomBytes >> 4) + 2 * k);
-            umma_ss_lo(tmem_S[t], q_lo[t] + off, k_lo + off, idesc_qk, (a | k) != 0);
-          }
-        }
-        umma_commit(&s_bar[t]);
-      };
-      auto issue_pv = [&](int t, int vstage, bool accumulate) {
-        // A = P_t from TMEM (bf16 pairs: 16 keys = 8 columns per UMMA_K step);
-        // B = V block, MN-major: 64-col halves LBO = kAtomBytes apart, 8-key groups 1024 B apart, 16 keys = 2048 B (+128)
-        const uint32_t v_lo = desc_lo_mnmajor(smem_u32(smem_kv + vstage * kTileBytes), kAtomBytes);
-#pragma unroll
-        for (int k = 0; k < kBlockN / 16; ++k)
-          umma_ts_lo(tmem_O[t], tmem_S[t] + k * 8, v_lo + (uint32_t)(k * (2048 >> 4)), idesc_pv, (accumulate || k != 0) ? 1u : 0u);
-      };
-
-      while (true) {
-        mbar_wait(&sched_full[slot], sphase);
-        const int item = sched_item[slot];
-        mbar_arrive(&sched_empty[slot]);
-        if (++slot == 2) { slot = 0; sphase ^= 1; }
-        if (item >= p.num_items) break;
-        const AttnItem w = attn_decode_item(item, p);
-        if (w.nblk == 0) continue;
-        const int nblk = w.nblk;
-        const int ntile = w.tile1_active ? 2 : 1;
-
-        mbar_wait(q_full, q_phase);
-        q_phase ^= 1;
-        // block 0 scores for both tiles (a tile with no visible key at all — causal, Lq > Lk — sweeps nothing)
-        mbar_wait(&kv_full[stage], phase);
-        tc_fence_after();
-        for (int t = 0; t < ntile; ++t)
-          if (w.nblk_t[t] > 0) issue_qk(t, stage);
-        umma_commit(&kv_empty[stage]);  // K_0 slot free once both S(0) are done
-        if (nblk == 1) umma_commit(q_empty);
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-
-        for (int j = 0; j < nblk; ++j) {
-          const int vstage = stage;
-          ATTN_TRACE(2, tr_it, 4);
-          mbar_wait(&kv_full[vstage], phase);  // V_j
+            tma_load_2d(smem_kv + stage * kTileBytes + a * kAtomBytes, tm, &kv_full[stage], hk * D + a * 64,
+                        k_beg + j * kBlockN, kEvictLast);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
-          const int kstage = stage;
-          const bool has_next = (j + 1) < nblk;
-          if (has_next) {
-            mbar_wait(&kv_full[kstage], phase);  // K_{j+1}
-            if (++stage == kStages) { stage = 0; phase ^= 1; }
-          }
-          tc_fence_after();
-          ATTN_TRACE(2, tr_it, 5);
-          for (int t = 0; t < ntile; ++t) {
-            if (j >= w.nblk_t[t]) continue;      // causal: this block lies entirely above the tile's diagonal
-            const bool t_next = (j + 1) < w.nblk_t[t];
-            ATTN_TRACE(2, tr_it, 0);
-            mbar_wait(&p_bar[t], pcnt[t] & 1);  // P_t(j) in TMEM, O_t rescaled
-            ATTN_TRACE(2, tr_it, 1);
-            ++pcnt[t];
-            if (j == 0) mbar_wait(&o_free[t], (icnt[t] & 1) ^ 1);   // the previous item's O_t has been read out
-            tc_fence_after();
-            issue_pv(t, vstage, j > 0);
-            if (!t_next) umma_commit(&o_bar[t]);
-            // S_t(j+1) overwrites the columns P_t(j) lives in: safe because the tensor pipe executes in issue order
-            if (t_next) issue_qk(t, kstage);
-            ATTN_TRACE(2, tr_it, 2);
-#ifdef BAGEL_ATTN_TRACE
-            if (blockIdx.x == 0 && tr_it < kTraceIters) g_attn_trace[(2 * kTraceIters + tr_it) * kTraceEvents + 3] = t;
-            ++tr_it;
-#endif
-          }
-          umma_commit(&kv_empty[vstage]);
-          if (has_next) umma_commit(&kv_empty[kstage]);
-          if (has_next && j + 2 == nblk) umma_commit(q_empty);   // that was the item's last QK^T
-          ATTN_TRACE(2, tr_it - 1, 6);
         }
-        for (int t = 0; t < ntile; ++t)
-          if (w.nblk_t[t] > 0) ++icnt[t];
       }
     }
   } else {
-    // =========================== softmax / correction / epilogue ===========================
-    const int t = warp / kSoftWarps;                 // which query tile this warp group serves
-    const int quarter = warp & 3;                    // TMEM lane quarter accessible to this warp
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_off = uint32_t(quarter * 32) << 16;
-    constexpr int NC = kBlockN;                      // score columns per thread
-    const uint32_t tS = tmem_S[t] + lane_off;
-    const uint32_t tP = tmem_S[t] + lane_off;        // packed bf16 probabilities over the first 64 columns of S
-    const uint32_t tO = tmem_O[t] + lane_off;
-    uint32_t scnt = 0;     // S blocks consumed by this tile (parity of s_bar)
-    uint32_t icnt = 0;     // items processed by this tile (parity of o_bar)
-    int slot = 0;
-    uint32_t sphase = 0;
-    [[maybe_unused]] int tr_it = 0;
-    [[maybe_unused]] const bool tr_on = (quarter == 0 && lane == 0);
+    // =========================== S = QK^T, online softmax, O += PV ===========================
+    const int half = wg;                                       // query rows [64 half, 64 half + 64) of the tile
+    const int cq = 2 * (lane & 3);                             // fragment column offset
+    const int row0 = half * 64 + (warp & 3) * 16 + (lane >> 2); // fragment rows row0 and row0 + 8
+    const int qi[2] = {q0 + row0, q0 + row0 + 8};              // query index within the sample
+    float o[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
-    while (true) {
-      mbar_wait(&sched_full[slot], sphase);
-      const int item = sched_item[slot];
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sched_empty[slot]);
-      if (++slot == 2) { slot = 0; sphase ^= 1; }
-      if (item >= p.num_items) break;
-      const AttnItem w = attn_decode_item(item, p);
-      if (!w.valid || (t == 1 && !w.tile1_active)) continue;
-      const int nblk = w.nblk_t[t];
-      const int Lq = w.Lq, Lk = w.Lk, shift = w.shift;
-      const int qi = w.q0 + t * kBlockM + row;  // query index within the sample
-
-      float m = -INFINITY, l = 0.f;
-      // Streamed online softmax. The stage is bound by instruction issue (one softmax warp of each tile per scheduler),
-      // so the hot loop is pared down to 6 instructions per PAIR of scores (FFMA2 scale/shift, 2x MUFU.EX2, FADD2 row sum,
-      // F2FP pack; no masking code in interior blocks, no max tracking). S is read in 32-column chunks; while chunk c+1 is
-      // in flight chunk c is exponentiated against the reference maximum `m` carried over from earlier blocks (lazy
-      // rescaling). Only when a row has no reference yet, or the row sum shows that m has become badly stale, is the
-      // block redone the classic way: exact block maximum, move m, rescale O and l, re-read S.
-      // Redo trigger of the streamed path: the block's row sum of p = 2^((s - m) scale). With an up-to-date m every p <= 1
-      // and the sum is <= 128; a stale m only scales p, l and O by a common power of two, which fp32 (and bf16, same
-      // exponent range) absorb without loss — so the maximum itself is NOT tracked in the hot loop (one FMNMX3 per pair
-      // of elements saved) and the block is redone exactly only when the sum says some p left the comfortable range
-      // (or overflowed: inf / NaN fail the comparison too). Exercised by tests/test_gpu_attn_adversarial.py.
-      constexpr float kRedoSum = 1073741824.0f;   // 2^30
+    if (nblk > 0) {
+      mbar_wait(q_full, 0);
+      const uint32_t q_addr = smem_u32(smem_q) + half * 64 * 128;
+      const int tile_q_lo = q0 + half * 64;
+      int stage = 0;
+      uint32_t phase = 0;
       for (int j = 0; j < nblk; ++j) {
-        if (tr_on) ATTN_TRACE(t, tr_it, 0);
-        mbar_wait(&s_bar[t], scnt & 1);
-        if (tr_on) ATTN_TRACE(t, tr_it, 1);
-        ++scnt;
-        tc_fence_after();
-        const int kv0 = j * kBlockN;               // first key of this block
-        const int tile_q_lo = w.q0 + t * kBlockM;
-        const bool need_mask = (j * kBlockN + kBlockN > Lk) || (p.causal && (j * kBlockN + kBlockN - 1 > tile_q_lo + shift));
-        const int lim = p.causal ? min(Lk - 1, qi + shift) : (Lk - 1);  // last visible key for this row
-
-        uint32_t pk[NC / 2];  // packed bf16 probabilities of this thread's columns (stored after S is fully read)
-        float2 rs2[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-        const float2 sc2 = make_float2(p.scale_log2, p.scale_log2);
-
-        // kMask is a compile-time tag: interior blocks (the vast majority) must not carry the predicated-off compare /
-        // select instructions of the masked variant — they still cost issue slots (310 of 700 per block and thread)
-        auto process_t = [&](auto mask_tag, auto poly_tag, const uint32_t (&v)[32], int c, float neg_ms) {
-          constexpr bool kMask = decltype(mask_tag)::value;
-          constexpr bool kPoly = decltype(poly_tag)::value && !kMask;
-          const float2 nm2 = make_float2(neg_ms, neg_ms);
+        // ---- S = Q K_j^T: K-major operands, D = kAtoms atoms of 64 columns, 4 k16 steps (+32 B) per atom ----
+        float s[kBlockN / 2];
+        mbar_wait(&kv_full[stage], phase);
+        {
+          const uint32_t k_addr = smem_u32(smem_kv + stage * kTileBytes);
+          wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float x0 = __uint_as_float(v[2 * i]), x1 = __uint_as_float(v[2 * i + 1]);
-            if constexpr (kMask) {
-              if (kv0 + c * 32 + 2 * i > lim) x0 = -INFINITY;
-              if (kv0 + c * 32 + 2 * i + 1 > lim) x1 = -INFINITY;
-            }
-            const float2 x = ffma2(make_float2(x0, x1), sc2, nm2);
-            const float2 e = (kPoly && (i & 3) == 3) ? ex2_poly2(x) : make_float2(ex2(x.x), ex2(x.y));
-            rs2[i & 1] = fadd2(rs2[i & 1], e);
-            pk[c * 16 + i] = pack_bf16x2(e.x, e.y);
-          }
-        };
-
-        // warp-uniform (tcgen05.ld is .sync.aligned): the streamed path needs a reference maximum in every row of the warp
-        const bool have_ref = __all_sync(0xffffffffu, m != -INFINITY);
-        bool redo = true;
-        if (have_ref) {
-          const float neg_ms = -m * p.scale_log2;
-          auto stream = [&](auto mask_tag, auto poly_tag) {
-            uint32_t va[32], vb[32];
-            tmem_ld_x32(tS + 0, va);
-            tmem_ld_wait();
+          for (int a = 0; a < kAtoms; ++a)
 #pragma unroll
-            for (int c = 0; c < NC / 32; c += 2) {
-              if (c + 1 < NC / 32) tmem_ld_x32(tS + (c + 1) * 32, vb);
-              process_t(mask_tag, poly_tag, va, c, neg_ms);
-              if (c + 1 < NC / 32) {
-                tmem_ld_wait();
-                if (c + 2 < NC / 32) tmem_ld_x32(tS + (c + 2) * 32, va);
-                process_t(mask_tag, poly_tag, vb, c + 1, neg_ms);
-                if (c + 2 < NC / 32) tmem_ld_wait();
-              }
-            }
-          };
-          // (A chunk-level classification of boundary blocks — skip the chunks no row of the warp can see, unmasked code for the
-          // chunks every row sees in full — was measured SLOWER than masking the whole block per element: it gives up the
-          // double-buffered loads and bloats the loop; profiles/r02_attn_halfrow_ab.txt, last section.)
-          if (need_mask) stream(std::true_type{}, std::false_type{});
-          else if (p.poly) stream(std::false_type{}, std::true_type{});
-          else stream(std::false_type{}, std::false_type{});
-          const float rs_row = (rs2[0].x + rs2[1].x) + (rs2[0].y + rs2[1].y);
-          redo = !(rs_row <= kRedoSum);
-          if (tr_on) ATTN_TRACE(t, tr_it, 2);
+            for (int k = 0; k < 4; ++k)
+              wgmma_ss<kBlockN>(s, gmma_desc_kmajor_sw128(q_addr + a * kAtomBytes) + 2 * k,
+                                gmma_desc_kmajor_sw128(k_addr + a * kAtomBytes) + 2 * k, (a | k) != 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          gmma_fence_operand(s);
         }
-        float alpha = 1.0f;
-        if (__any_sync(0xffffffffu, redo)) {
-          // slow path (first block of a row, or a large jump of the maximum): classic two-pass on re-reads of S, one
-          // 32-column chunk in registers at a time (rare, so latency matters less than register pressure)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&kv_empty[stage]);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+
+        // ---- online softmax over this thread's two rows (a row's 128 scores are spread over a lane quad) ----
+        const int kv0 = j * kBlockN;
+        const bool need_mask = (kv0 + kBlockN > Lk) || (p.causal && (kv0 + kBlockN - 1 > tile_q_lo + shift));
+        if (need_mask) {
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int lim = p.causal ? min(Lk - 1, qi[r] + shift) : (Lk - 1);   // last visible key of this row
+#pragma unroll
+            for (int c = 0; c < kBlockN / 8; ++c)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                if (kv0 + 8 * c + cq + e > lim) s[4 * c + 2 * r + e] = -INFINITY;
+          }
+        }
+        float neg_ms[2], alpha[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
           float mx = -INFINITY;
-#pragma unroll 1
-          for (int c = 0; c < NC / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld_x32(tS + c * 32, v);
-            tmem_ld_wait();
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              float x = __uint_as_float(v[i]);
-              if (need_mask && (kv0 + c * 32 + i > lim)) x = -INFINITY;
-              mx = fmaxf(mx, x);
-            }
-          }
-          float neg_ms = -m * p.scale_log2;
-          if (redo) {
-            const float m_new = fmaxf(m, mx);
-            const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-            alpha = ex2((m - m_use) * p.scale_log2);  // m = -inf -> 0
-            m = m_new;
-            neg_ms = -m_use * p.scale_log2;
-            rs2[0] = make_float2(0.f, 0.f);
-            rs2[1] = make_float2(0.f, 0.f);
-          }
+          for (int c = 0; c < kBlockN / 8; ++c) mx = fmaxf(mx, fmaxf(s[4 * c + 2 * r], s[4 * c + 2 * r + 1]));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          const float m_new = fmaxf(m[r], mx);
+          const float m_use = (m_new == -INFINITY) ? 0.f : m_new;   // a row with no visible key yet: p = 0
+          alpha[r] = ex2((m[r] - m_use) * p.scale_log2);            // m = -inf -> 0
+          m[r] = m_new;
+          neg_ms[r] = -m_use * p.scale_log2;
+        }
+        // P = 2^(s scale - m scale) as bf16 A fragments of the P*V wgmma: keys 16kk .. 16kk + 15 are column blocks
+        // 2kk (a0: row0, a1: row0 + 8) and 2kk + 1 (a2, a3)
+        const bool poly = p.poly && !need_mask;
+        float rs[2] = {0.f, 0.f};
+        uint32_t pa[kBlockN / 16][4];
 #pragma unroll
-          for (int c = 0; c < NC / 32; ++c) {  // all lanes load (sync.aligned); only the rows that moved recompute
-            uint32_t v[32];
-            tmem_ld_x32(tS + c * 32, v);
-            tmem_ld_wait();
-            if (redo) {
-              if (need_mask) process_t(std::true_type{}, std::false_type{}, v, c, neg_ms);
-              else process_t(std::false_type{}, std::false_type{}, v, c, neg_ms);
-            }
-          }
-          if (j > 0) {  // O_t(j-1) is complete: S_t(j) was issued after PV_t(j-1) and the pipe is in-order
+        for (int c = 0; c < kBlockN / 8; ++c) {
 #pragma unroll
-            for (int c = 0; c < D / 32; ++c) {
-              uint32_t v[32];
-              tmem_ld_x32(tO + c * 32, v);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-              tmem_st_x32(tO + c * 32, v);
-            }
+          for (int r = 0; r < 2; ++r) {
+            const float2 x = make_float2(fmaf(s[4 * c + 2 * r], p.scale_log2, neg_ms[r]),
+                                         fmaf(s[4 * c + 2 * r + 1], p.scale_log2, neg_ms[r]));
+            const float2 e = (poly && (c & 3) == 3) ? ex2_poly2(x) : make_float2(ex2(x.x), ex2(x.y));
+            rs[r] += e.x + e.y;
+            pa[c >> 1][(c & 1) * 2 + r] = pack_bf16x2(e.x, e.y);
           }
         }
-        const float rs = (rs2[0].x + rs2[1].x) + (rs2[0].y + rs2[1].y);
-        l = l * alpha + rs;
-        // P (bf16 pairs) over the first 64 columns of the S region: all of S has been read by now
 #pragma unroll
-        for (int c = 0; c < NC / 64; ++c)
-          tmem_st_x32(tP + c * 32, *reinterpret_cast<const uint32_t(*)[32]>(&pk[c * 32]));
-        tmem_st_wait();
-        if (tr_on) ATTN_TRACE(t, tr_it, 3);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_bar[t]);
-        if (tr_on) ATTN_TRACE(t, tr_it, 4);
-#ifdef BAGEL_ATTN_TRACE
-        ++tr_it;
-#endif
-      }
+        for (int r = 0; r < 2; ++r) {
+          l[r] = l[r] * alpha[r] + rs[r];
+#pragma unroll
+          for (int c = 0; c < D / 8; ++c) {
+            o[4 * c + 2 * r] *= alpha[r];
+            o[4 * c + 2 * r + 1] *= alpha[r];
+          }
+        }
 
-      // ---- epilogue: O / l -> bf16 -> global ----
-      if (nblk > 0) {
-        mbar_wait(&o_bar[t], icnt & 1);
-        ++icnt;
-        tc_fence_after();
-      }
-      // rows that never saw a visible key (m still -inf) produce 0, as flash-attn does
-      const float inv_l = (l > 0.f && m != -INFINITY) ? (1.f / l) : 0.f;
-      const bool row_ok = qi < Lq;
-      __nv_bfloat16* orow = p.out + (long long)(w.q_beg + qi) * p.ld_out + w.h * D;
+        // ---- O += P V_j: B = V block, MN-major (64-column halves kAtomBytes apart), 16 keys = 2048 B per k16 step ----
+        mbar_wait(&kv_full[stage], phase);
+        {
+          const uint32_t v_addr = smem_u32(smem_kv + stage * kTileBytes);
+          wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < D / 32; ++c) {
-        uint32_t v[32];
-        if (nblk > 0) {
-          tmem_ld_x32(tO + c * 32, v);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = 0u;
+          for (int kk = 0; kk < kBlockN / 16; ++kk)
+            wgmma_rs<D, 1>(o, pa[kk], gmma_desc_mnmajor_sw128(v_addr + kk * 2048, kAtomBytes), 1u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          gmma_fence_operand(o);
         }
-        if (row_ok) {
-          uint4* dst = reinterpret_cast<uint4*>(orow + c * 32);
-#pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4) {
-            uint32_t o[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              o[e] = pack_bf16x2(__uint_as_float(v[q4 * 8 + 2 * e]) * inv_l, __uint_as_float(v[q4 * 8 + 2 * e + 1]) * inv_l);
-            dst[q4] = make_uint4(o[0], o[1], o[2], o[3]);
-          }
-        }
-      }
-      if (nblk > 0) {   // O_t is in registers / memory: the next item's first P*V may overwrite the accumulator
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) mbar_arrive(&o_free[t]);
+        if (lane == 0) mbar_arrive(&kv_empty[stage]);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
     }
-  }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+    // ---- epilogue: O / l -> bf16 -> global; rows that never saw a visible key produce 0, as flash-attn does ----
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float lr = l[r];
+      lr += __shfl_xor_sync(0xffffffffu, lr, 1);
+      lr += __shfl_xor_sync(0xffffffffu, lr, 2);
+      const float inv_l = (lr > 0.f && m[r] != -INFINITY) ? (1.f / lr) : 0.f;
+      if (qi[r] >= Lq) continue;
+      __nv_bfloat16* orow = p.out + (long long)(q_beg + qi[r]) * p.ld_out + h * D;
+#pragma unroll
+      for (int c = 0; c < D / 8; ++c)
+        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = pack_bf16x2(o[4 * c + 2 * r] * inv_l, o[4 * c + 2 * r + 1] * inv_l);
+    }
   }
-}
-
-// device counters of the work-item scheduler: a small ring so that back-to-back launches (and launches captured in a CUDA
-// graph together with their memset node) never share a counter that is still in use
-static int* sched_counter(cudaStream_t stream) {
-  constexpr int kRing = 64;
-  static int* base[64] = {nullptr};
-  static std::atomic<unsigned> next{0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return nullptr;
-  if (base[dev] == nullptr) {
-    int* ptr = nullptr;
-    if (cudaMalloc(&ptr, kRing * sizeof(int)) != cudaSuccess) return nullptr;
-    base[dev] = ptr;
-  }
-  int* c = base[dev] + (next.fetch_add(1, std::memory_order_relaxed) % kRing);
-  if (cudaMemsetAsync(c, 0, sizeof(int), stream) != cudaSuccess) return nullptr;
-  return c;
 }
 
 template <int D>
-static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, AttnParams p, int B,
+static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p, int B,
                        int max_seqlen_q, cudaStream_t stream) {
   using Cfg = AttnCfg<D>;
   auto kern = attn_varlen_kernel<D>;
@@ -666,14 +285,9 @@ static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUt
     BAGEL_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_done = true;
   }
-  p.qtiles = (max_seqlen_q + 2 * kBlockM - 1) / (2 * kBlockM);
-  const long long items = (long long)p.qtiles * p.Hq * B;
-  if (items > 0x7fffffff - 4096) return set_error(BAGEL_ERR_SHAPE, "bagel_attn_varlen_fwd: too many work items");
-  p.num_items = (int)items;
-  p.sched = sched_counter(stream);
-  if (p.sched == nullptr) return set_error(BAGEL_ERR_CUDA, "bagel_attn_varlen_fwd: scheduler counter allocation failed");
-  const int grid = p.num_items < sm_count() ? p.num_items : sm_count();
-  kern<<<grid, kAttnThreads, Cfg::kSmemBytes, stream>>>(tmQ, tmK, tmV, p);
+  const int qtiles = (max_seqlen_q + kBlockM - 1) / kBlockM;
+  if (p.Hq > 65535 || B > 65535) return set_error(BAGEL_ERR_SHAPE, "bagel_attn_varlen_fwd: too many heads / samples");
+  kern<<<dim3(qtiles, p.Hq, B), kAttnThreads, Cfg::kSmemBytes, stream>>>(tmQ, tmK, tmV, p);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   BAGEL_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -682,13 +296,6 @@ static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUt
 }  // namespace bagel
 
 using namespace bagel;
-
-#ifdef BAGEL_ATTN_TRACE
-extern "C" int bagel_attn_trace_read(long long* host, int n) {
-  cudaDeviceSynchronize();
-  return (int)cudaMemcpyFromSymbol(host, g_attn_trace, sizeof(long long) * n);
-}
-#endif
 
 extern "C" int bagel_attn_varlen_fwd(const void* q, const void* k, const void* v, void* out, const int* cu_seqlens_q,
                                      const int* cu_seqlens_k, int total_q, int total_k, int batch, int num_heads_q,
@@ -702,9 +309,9 @@ extern "C" int bagel_attn_varlen_fwd(const void* q, const void* k, const void* v
   if (batch <= 0 || total_q < 0 || total_k < 0) return set_error(BAGEL_ERR_SHAPE, "bagel_attn_varlen_fwd: bad sizes");
   if ((ld_q % 8) || (ld_k % 8) || (ld_v % 8) || (ld_out % 8) || (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15))
     return set_error(BAGEL_ERR_ALIGN, "bagel_attn_varlen_fwd: row strides %% 8 and 16-byte aligned pointers required");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   if (total_q == 0 || max_seqlen_q <= 0) return 0;
-  // one query token per sample (text decode): HBM-bound split-KV kernel instead of the 128-row tcgen05 tiles.
+  // one query token per sample (text decode): HBM-bound split-KV kernel instead of the 128-row wgmma tiles.
   // A single query sees every key under both mask settings (bottom-right aligned causal), so `causal` is moot.
   if (attn_decode_supported(max_seqlen_q, head_dim, num_heads_q, num_heads_k))
     return attn_decode(q, k, v, out, cu_seqlens_q, cu_seqlens_k, seqused_k, batch, num_heads_q, num_heads_k,
@@ -716,10 +323,6 @@ extern "C" int bagel_attn_varlen_fwd(const void* q, const void* k, const void* v
   if (int rc = make_tmap_2d_bf16(&tmK, k, (uint64_t)num_heads_k * head_dim, rows_k, (uint64_t)ld_k, 64, kBlockN)) return rc;
   if (int rc = make_tmap_2d_bf16(&tmV, v, (uint64_t)num_heads_k * head_dim, rows_k, (uint64_t)ld_v, 64, kBlockN)) return rc;
 
-  if (attn3_enabled())
-    return attn3_varlen(tmQ, tmK, tmV, out, ld_out, cu_seqlens_q, cu_seqlens_k, seqused_k, batch, num_heads_q, num_heads_k,
-                        head_dim, max_seqlen_q, causal, softmax_scale * 1.4426950408889634f, static_cast<cudaStream_t>(stream));
-
   AttnParams p{};
   p.out = static_cast<__nv_bfloat16*>(out);
   p.ld_out = ld_out;
@@ -730,10 +333,10 @@ extern "C" int bagel_attn_varlen_fwd(const void* q, const void* k, const void* v
   p.Hk = num_heads_k;
   p.causal = causal;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
-  // FMA-pipe exp2 for every 4th score pair: +2-6 % on long non-causal sweeps (denoise, ViT), neutral to -9 % on short causal
-  // ones (profiles/r02_attn_poly_stages_ab.txt) -> on for non-causal calls; BAGEL_ATTN_POLY=0/1 forces it off / on
+  // FMA-pipe exp2 for every 4th score pair: on for long non-causal sweeps (denoise, ViT at >= 2k keys), where MUFU limits the
+  // softmax; off for short or causal ones, where it measured slower; BAGEL_ATTN_POLY=0/1 forces it off / on
   static const int poly_env = [] { const char* e = getenv("BAGEL_ATTN_POLY"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
-  p.poly = poly_env >= 0 ? poly_env : (causal ? 0 : 1);
+  p.poly = poly_env >= 0 ? poly_env : ((causal || max_seqlen_k < 2048) ? 0 : 1);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (head_dim == 128) return launch_attn<128>(tmQ, tmK, tmV, p, batch, max_seqlen_q, s);
   return launch_attn<64>(tmQ, tmK, tmV, p, batch, max_seqlen_q, s);

@@ -3,7 +3,7 @@
 // qwen2_navit.py:579-588 with causal=True, one new token against the whole cache).
 //
 // This is an HBM-bound stream over the K/V cache (2 * len * Hk * 128 * 2 bytes per sample), not a GEMM: the
-// tcgen05 kernel in attn.cu would spend a 128-row query tile (and a whole CTA) on one valid row per q head and
+// wgmma kernel in attn.cu would spend a 128-row query tile (and a whole CTA) on one valid row per q head and
 // walk the keys serially. Here instead:
 //   * grid = (split, Hk, batch): the keys of one (sample, kv head) are split over the CTAs of a thread-block
 //     CLUSTER; each CTA handles all G = Hq/Hk query heads that share the kv head, so K and V are read exactly once;

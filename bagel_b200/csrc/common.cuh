@@ -1,11 +1,13 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM).
-// Everything here is a device-side primitive used by gemm.cu / attn.cu; no CUTLASS dependency.
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
+// Everything here is a device-side primitive used by gemm.cu / gemm_skinny.cu / attn.cu; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "wgmma.cuh"
 
 namespace bagel {
 
@@ -71,10 +73,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// Exactly one lane of a CONVERGED warp. Use this — not `lane == 0` — to guard single-thread tcgen05 / TMA issue: with
-// elect.sync ptxas knows one thread runs the region and keeps descriptors on the uniform datapath (UIADD3 + back-to-back
-// UTCHMMA). Behind `lane == 0` it wraps EVERY tcgen05.mma in ELECT / 4-5 x R2UR.BROADCAST / PLOP3 / BRA.U.ANY, ~80 cycles of
-// dependent instruction stream per MMA (measured in the attention kernel, whose 64-cycle MMAs it paced).
+// Exactly one lane of a CONVERGED warp (elect.sync): guards single-thread TMA issue; with it ptxas knows that one thread
+// runs the region, behind `lane == 0` it has to assume divergence.
 __device__ __forceinline__ bool elect_one_lane() {
   uint32_t pred;
   asm volatile(
@@ -93,7 +93,7 @@ __device__ __forceinline__ bool elect_one_lane() {
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// generic-proxy smem writes -> visible to the async proxy (TMA / UMMA operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -144,177 +144,62 @@ __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, ld/st, fences
+// wgmma: shared-memory matrix descriptors, fences, the M = 64 warpgroup MMA
 // ---------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "pow2 >= 32");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Shared-memory matrix descriptor (PTX "matrix-descriptor", sm_90 wgmma flavour):
+//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base_offset | [62,64) layout (1 = SWIZZLE_128B)
+// K-major SWIZZLE_128B operand tile: rows are 128 B apart, 8-row groups are 1024 B apart (SBO); LBO unused (1).
+// Advancing 16 elements (32 B) along K inside the 128 B swizzle atom is +2 in the start field.
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Shared-memory matrix descriptor (PTX "matrix-descriptor", tcgen05 flavour):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [49,52) base_offset | [61,64) swizzle
-// K-major SWIZZLE_128B operand tile: rows are 128 B apart, 8-row groups are 1024 B apart (SBO); LBO unused.
-constexpr uint64_t kSwz128 = 2;
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (kSwz128 << 61);
-}
-// MN-major SWIZZLE_128B operand tile (used for V in P*V): along MN 64 elements (128 B) are contiguous and the
-// next 64-element block is LBO bytes away; along K rows are 128 B apart, 8-row groups SBO (=1024) apart.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
+// MN-major SWIZZLE_128B operand tile (V in P*V): along MN 64 elements (128 B) are contiguous and the next 64-element
+// block is LBO bytes away; along K rows are 128 B apart, 8-row groups SBO (= 1024) apart.
+__device__ __forceinline__ uint64_t gmma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
   return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (kSwz128 << 61);
+         ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
-// Instruction descriptor for kind::f16, BF16 x BF16 -> F32.
-//   [4,6) D fmt (1=f32) | [7,10) A fmt (1=bf16) | [10,13) B fmt | 15 A major | 16 B major (0=K,1=MN)
-//   [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+// Register operands of an in-flight wgmma must not be touched (or moved) by the compiler until wgmma_wait retires it.
+template <int N>
+__device__ __forceinline__ void gmma_fence_operand(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands in shared memory; issued by all 128 threads of a warpgroup.
+template <int N, int kTnspB = 0>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  if constexpr (N == 16) wgmma_ss_n16<kTnspB>(d, a_desc, b_desc, scale_d);
+  else if constexpr (N == 32) wgmma_ss_n32<kTnspB>(d, a_desc, b_desc, scale_d);
+  else if constexpr (N == 64) wgmma_ss_n64<kTnspB>(d, a_desc, b_desc, scale_d);
+  else if constexpr (N == 128) wgmma_ss_n128<kTnspB>(d, a_desc, b_desc, scale_d);
+  else {
+    static_assert(N == 256, "wgmma_ss: N in {16, 32, 64, 128, 256}");
+    wgmma_ss_n256<kTnspB>(d, a_desc, b_desc, scale_d);
+  }
 }
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// D[64 x N] (+)= A[64 x 16] (registers) * B[16 x N] (shared memory)
+template <int N, int kTnspB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  if constexpr (N == 64) wgmma_rs_n64<kTnspB>(d, a, b_desc, scale_d);
+  else {
+    static_assert(N == 128, "wgmma_rs: N in {64, 128}");
+    wgmma_rs_n128<kTnspB>(d, a, b_desc, scale_d);
+  }
 }
 
-// TMEM -> registers, shape 32x32b: lane (= accumulator row) per thread, N consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-      "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-      "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------
-// CTA pair (cta_group::2): two CTAs of a 2-CTA cluster (same TPC) execute ONE tcgen05.mma of M = 256 — each CTA holds
-// its own 128 rows of A, HALF of the B tile (N/2 rows) and its 128 accumulator rows in its own TMEM. Only the leader
-// (cluster rank 0) issues MMAs; both CTAs issue TMA loads, all of which complete on the LEADER's full barrier.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem offset in the pair's leader CTA (bit 24 = rank within the pair)
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-// TMA load issued by either CTA of the pair into ITS OWN shared memory; the transaction bytes are counted on the leader's
-// mbarrier (same offset, peer bit cleared).
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1,
-                                                uint64_t hint) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst) {   // one warp of EACH CTA of the pair, same smem offset
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(kCols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem of both CTAs, 128 rows each] * B[smem of both CTAs, N/2 rows each]; leader only.
-__device__ __forceinline__ void umma_ss_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once all previously issued MMAs of this thread retire) on the mbarrier at this smem offset in every CTA of
-// `cta_mask` (bit i = cluster rank i).
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// mbarrier.arrive on the barrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
+// Warp-specialised kernels: the producer warpgroup gives registers back, the MMA warpgroups take them.
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 
 // ---------------------------------------------------------------------------------------------
 // numerics helpers: explicit bf16 rounding points (the reference's autocast casts, SURVEY.md §8a)

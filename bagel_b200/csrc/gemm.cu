@@ -1,15 +1,15 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:  C[M,N] = epilogue( A[M,K] * W[N,K]^T )
+// Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = epilogue( A[M,K] * W[N,K]^T )
 //
 // Replaces every nn.Linear on BAGEL's forward path (reference: modeling/bagel/qwen2_navit.py:515-517,
 // 529-536, 589-594; modeling/qwen2/modeling_qwen2.py:200-201; modeling/bagel/bagel.py:801-833), which
 // the reference runs as cuBLASLt GEMM + separate ATen elementwise launches.
 //
-//   warp 0      : TMA producer   (cp.async.bulk.tensor 2D, 128B swizzle, kStages-deep smem ring)
-//   warp 1      : MMA issuer     (one elected lane issues tcgen05.mma 128 x BN x 16, fp32 accum in TMEM)
-//   warps 2..5  : epilogue       (tcgen05.ld 32x32b -> registers -> fused epilogue -> global)
+//   warpgroup 0    : TMA producer (one elected lane: cp.async.bulk.tensor 2D, 128B swizzle, kStages-deep smem ring)
+//   warpgroups 1-2 : MMA + epilogue, 64 rows of the 128 x BN tile each (wgmma m64nBNk16, fp32 accumulators in
+//                    registers, one wgmma group kept in flight), fused epilogue straight from the accumulator fragments
 //
-// TMEM holds two accumulator stages (2 x BN columns) so the epilogue of tile i overlaps the MMAs of tile
-// i+1. A and W are both K-major ("TN" GEMM: nn.Linear weight layout), fp32 accumulation, bf16 output.
+// The producer runs ahead into the next tile of the persistent loop while the MMA warpgroups are in their epilogue.
+// A and W are both K-major ("TN" GEMM: nn.Linear weight layout), fp32 accumulation, bf16 output.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -21,7 +21,6 @@
 #include "host_util.h"
 #include "gemm_skinny.h"
 #include "gemm_params.h"
-#include "gemm2.h"
 
 namespace bagel {
 
@@ -48,37 +47,28 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint8_t* smem_b = smem + kStages * Cfg::kABytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
   uint64_t* full_bar = bars;                  // [kStages]  TMA -> MMA
-  uint64_t* empty_bar = bars + kStages;       // [kStages]  MMA -> TMA
-  uint64_t* tfull_bar = bars + 2 * kStages;   // [2]        MMA -> epilogue
-  uint64_t* tempty_bar = tfull_bar + 2;       // [2]        epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* empty_bar = bars + kStages;       // [kStages]  MMA -> TMA (one arrive per MMA warp)
 
+  const int wg = threadIdx.x >> 7;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_k = CONV ? p.ksize * p.ksize * p.cin_chunks : (p.K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 4);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[i], kGemmMmaWarps);
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (elect_one_lane()) {   // not `lane == 0`: see common.cuh
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one_lane()) {
       int stage = 0;
       uint32_t phase = 0;
       const uint64_t hint_a = (p.hints & 2) ? kEvictFirst : ((p.hints & 8) ? kEvictLast : kEvictNormal);
@@ -107,200 +97,122 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one_lane()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);  // epilogue has drained this accumulator stage
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t a_desc = umma_desc_kmajor_sw128(smem_u32(smem_a + stage * Cfg::kABytes));
-          const uint64_t b_desc = umma_desc_kmajor_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            // advance 16 elements (32 B) along K inside the 128 B swizzle atom: +2 in the (addr>>4) field
-            umma_ss(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (kb | k) != 0);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs retire
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);  // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // ===================== epilogue warps (2..5) =====================
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may access
-    const int row_in_tile = quarter * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== MMA + epilogue warpgroups (1, 2) =====================
+    setmaxnreg_inc<232>();
+    const int half = wg - 1;                      // rows [64 * half, 64 * half + 64) of every tile
+    const int wq = warp & 3;                      // warp within the warpgroup: fragment rows 16 wq .. 16 wq + 15
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       int m_blk, n_blk;
       tile_coords(tile, p.num_m, p.num_n, p.group_m, p.group_n, m_blk, n_blk);
-      int row;
-      bool row_ok;
-      long long out_row;
-      if constexpr (CONV) {
-        const int tiles_img = p.tiles_w * p.tiles_h;
-        const int img = m_blk / tiles_img, t_in = m_blk - img * tiles_img;
-        const int ho = (t_in / p.tiles_w) * p.th + row_in_tile / p.tw;
-        const int wo = (t_in % p.tiles_w) * p.tw + row_in_tile % p.tw;
-        row_ok = (ho < p.Ho) && (wo < p.Wo);
-        row = (img * p.Ho + ho) * p.Wo + wo;
-        out_row = row;
-      } else {
-        row = m_blk * BM + row_in_tile;
-        row_ok = row < p.M;
-        out_row = row;
-        if (p.row_map != nullptr && row_ok) out_row = p.row_map[row];
+      float acc[BN / 2];
+      int prev = 0;
+      for (int kb = 0; kb < num_k; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_desc = gmma_desc_kmajor_sw128(smem_u32(smem_a + stage * Cfg::kABytes + half * 64 * 128));
+        const uint64_t b_desc = gmma_desc_kmajor_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / WGMMA_K; ++k) wgmma_ss<BN>(acc, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+        wgmma_commit();
+        if (kb > 0) {   // the previous k block's MMAs have retired: its smem slot may be refilled
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+      gmma_fence_operand(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_acc = tmem_base + acc * BN + (uint32_t(quarter * 32) << 16);
-
+      // epilogue: this thread holds rows r0 = 16 wq + lane / 4 and r0 + 8 (of its 64-row half), columns 8c + 2 (lane % 4) + {0, 1}
+      const int cq = 2 * (lane & 3);
       if constexpr (EPI == EPI_QKV) {
         static_assert(BN == 256, "fused QKV epilogue: two 128-wide heads per tile");
-        qkv_epilogue_row(p, t_acc, n_blk, row_ok, out_row);
-      } else if constexpr (EPI == EPI_SWIGLU) {
-        const int n_out0 = n_blk * (BN / 2);
-        __nv_bfloat16* crow = p.C + out_row * p.ldc + n_out0;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t g[32], u[32];
-          tmem_ld_x32(t_acc + c * 32, g);
-          tmem_ld_x32(t_acc + 128 + c * 32, u);
-          tmem_ld_wait();
-          if (row_ok) {
-            uint32_t o[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float h0, h1;
-              {
-                const float gg = bf16_round(__uint_as_float(g[2 * j]));
-                const float uu = bf16_round(__uint_as_float(u[2 * j]));
-                h0 = bf16_round(silu_f(gg)) * uu;
-              }
-              {
-                const float gg = bf16_round(__uint_as_float(g[2 * j + 1]));
-                const float uu = bf16_round(__uint_as_float(u[2 * j + 1]));
-                h1 = bf16_round(silu_f(gg)) * uu;
-              }
-              o[j] = pack_bf16x2(h0, h1);
-            }
-            const int n0 = n_out0 + c * 32;
-            if (n0 + 32 <= p.N / 2) {
-              uint4* dst = reinterpret_cast<uint4*>(crow + c * 32);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) store16(dst + q, make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]), p.hints & 4);
-            } else {
-              for (int j = 0; j < 16; ++j)
-                if (n0 + 2 * j < p.N / 2) *reinterpret_cast<uint32_t*>(crow + c * 32 + 2 * j) = o[j];
-            }
-          }
+        for (int h = 0; h < 2; ++h) {
+          const int row = m_blk * BM + half * 64 + wq * 16 + (lane >> 2) + 8 * h;
+          const bool row_ok = row < p.M;
+          const long long out_row = (row_ok && p.row_map != nullptr) ? (long long)p.row_map[row] : (long long)row;
+          qkv_epilogue_rows(p, acc, h, cq, n_blk, row_ok, out_row);
         }
       } else {
-        const int n0_tile = n_blk * BN;
-        __nv_bfloat16* crow = p.C + out_row * p.ldc + n0_tile;
-        const __nv_bfloat16* rrow = (EPI == EPI_RESID) ? p.resid + out_row * p.ldr + n0_tile : nullptr;
-        const float* rrow32 = (EPI == EPI_RESID_F32) ? p.resid32 + out_row * p.ldr + n0_tile : nullptr;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld_x32(t_acc + c * 32, v);
-          tmem_ld_wait();
-          const int n0 = n0_tile + c * 32;
-          if (row_ok && n0 < p.N) {
-            const bool full = (n0 + 32 <= p.N);
-            uint32_t rr[16];
-            if constexpr (EPI == EPI_RESID) {
-              if (full) {
-                const uint4* src = reinterpret_cast<const uint4*>(rrow + c * 32);
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const uint4 t = src[q];
-                  rr[4 * q] = t.x; rr[4 * q + 1] = t.y; rr[4 * q + 2] = t.z; rr[4 * q + 3] = t.w;
-                }
-              } else {
-                for (int j = 0; j < 16; ++j)
-                  rr[j] = (n0 + 2 * j < p.N) ? *reinterpret_cast<const uint32_t*>(rrow + c * 32 + 2 * j) : 0u;
-              }
+      for (int h = 0; h < 2; ++h) {
+        const int row_in_tile = half * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        bool row_ok;
+        long long out_row;
+        if constexpr (CONV) {
+          const int tiles_img = p.tiles_w * p.tiles_h;
+          const int img = m_blk / tiles_img, t_in = m_blk - img * tiles_img;
+          const int ho = (t_in / p.tiles_w) * p.th + row_in_tile / p.tw;
+          const int wo = (t_in % p.tiles_w) * p.tw + row_in_tile % p.tw;
+          row_ok = (ho < p.Ho) && (wo < p.Wo);
+          out_row = (long long)(img * p.Ho + ho) * p.Wo + wo;
+        } else {
+          const int row = m_blk * BM + row_in_tile;
+          row_ok = row < p.M;
+          out_row = row;
+          if (p.row_map != nullptr && row_ok) out_row = p.row_map[row];
+        }
+        if (!row_ok) continue;
+        if constexpr (EPI == EPI_SWIGLU) {
+          const int n_out0 = n_blk * (BN / 2);
+          __nv_bfloat16* crow = p.C + out_row * p.ldc + n_out0;
+#pragma unroll
+          for (int c = 0; c < 16; ++c) {
+            const int n = 8 * c + cq;
+            if (n_out0 + n >= p.N / 2) continue;
+            const float g0 = bf16_round(acc[4 * c + 2 * h]), g1 = bf16_round(acc[4 * c + 2 * h + 1]);
+            const float u0 = bf16_round(acc[4 * (c + 16) + 2 * h]), u1 = bf16_round(acc[4 * (c + 16) + 2 * h + 1]);
+            store4(crow + n, pack_bf16x2(bf16_round(silu_f(g0)) * u0, bf16_round(silu_f(g1)) * u1), p.hints & 4);
+          }
+        } else {
+          const int n0_tile = n_blk * BN;
+          __nv_bfloat16* crow = p.C + out_row * p.ldc + n0_tile;
+          const __nv_bfloat16* rrow = (EPI == EPI_RESID) ? p.resid + out_row * p.ldr + n0_tile : nullptr;
+          const float* rrow32 = (EPI == EPI_RESID_F32) ? p.resid32 + out_row * p.ldr + n0_tile : nullptr;
+          float* crow32 = (EPI == EPI_F32 || EPI == EPI_RESID_F32) ? p.C32 + out_row * p.ldc + n0_tile : nullptr;
+#pragma unroll
+          for (int c = 0; c < BN / 8; ++c) {
+            const int n = 8 * c + cq;              // N % 8 == 0: a column pair is in or out together
+            if (n0_tile + n >= p.N) continue;
+            float x0 = acc[4 * c + 2 * h], x1 = acc[4 * c + 2 * h + 1];
+            if (p.bias != nullptr) {
+              const uint32_t bb = *reinterpret_cast<const uint32_t*>(p.bias + n0_tile + n);
+              x0 += bf16_lo(bb);
+              x1 += bf16_hi(bb);
             }
-            uint32_t o[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float x0 = __uint_as_float(v[2 * j]);
-              float x1 = __uint_as_float(v[2 * j + 1]);
-              if (p.bias != nullptr) {
-                const int nb = min(n0 + 2 * j, p.N - 2);
-                const uint32_t bb = *reinterpret_cast<const uint32_t*>(p.bias + nb);
-                x0 += bf16_lo(bb);
-                x1 += bf16_hi(bb);
-              }
-              if constexpr (EPI == EPI_RESID) {
-                x0 = bf16_lo(rr[j]) + bf16_round(x0);
-                x1 = bf16_hi(rr[j]) + bf16_round(x1);
-              } else if constexpr (EPI == EPI_RESID_F32) {
-                if (n0 + 2 * j < p.N) {   // N % 8 == 0, so a pair is in or out together
-                  const float2 r2 = *reinterpret_cast<const float2*>(rrow32 + c * 32 + 2 * j);
-                  x0 = __fadd_rn(r2.x, bf16_round(x0));
-                  x1 = __fadd_rn(r2.y, bf16_round(x1));
-                }
-              } else if constexpr (EPI == EPI_GELU) {
-                x0 = gelu_tanh_f(bf16_round(x0));
-                x1 = gelu_tanh_f(bf16_round(x1));
-              } else if constexpr (EPI == EPI_SILU) {
-                x0 = silu_f(bf16_round(x0));
-                x1 = silu_f(bf16_round(x1));
-              }
-              if constexpr (EPI == EPI_F32 || EPI == EPI_RESID_F32) {
-                v[2 * j] = __float_as_uint(x0);     // reuse the accumulator registers for the fp32 result
-                v[2 * j + 1] = __float_as_uint(x1);
-              }
-              o[j] = pack_bf16x2(x0, x1);
+            if constexpr (EPI == EPI_RESID) {
+              const uint32_t rr = *reinterpret_cast<const uint32_t*>(rrow + n);
+              x0 = bf16_lo(rr) + bf16_round(x0);
+              x1 = bf16_hi(rr) + bf16_round(x1);
+            } else if constexpr (EPI == EPI_RESID_F32) {
+              const float2 r2 = *reinterpret_cast<const float2*>(rrow32 + n);
+              x0 = __fadd_rn(r2.x, bf16_round(x0));
+              x1 = __fadd_rn(r2.y, bf16_round(x1));
+            } else if constexpr (EPI == EPI_GELU) {
+              x0 = gelu_tanh_f(bf16_round(x0));
+              x1 = gelu_tanh_f(bf16_round(x1));
+            } else if constexpr (EPI == EPI_SILU) {
+              x0 = silu_f(bf16_round(x0));
+              x1 = silu_f(bf16_round(x1));
             }
             if constexpr (EPI == EPI_F32 || EPI == EPI_RESID_F32) {
-              float* d32 = p.C32 + out_row * p.ldc + n0;   // 128 contiguous bytes of this thread's row: 16-byte stores
-              if (full) {
-#pragma unroll
-                for (int q = 0; q < 8; ++q)
-                  reinterpret_cast<uint4*>(d32)[q] = make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-              } else {
-                for (int j = 0; j < 32; ++j)
-                  if (n0 + j < p.N) d32[j] = __uint_as_float(v[j]);
-              }
-            } else if (full) {
-              uint4* dst = reinterpret_cast<uint4*>(crow + c * 32);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) store16(dst + q, make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]), p.hints & 4);
+              *reinterpret_cast<float2*>(crow32 + n) = make_float2(x0, x1);
             } else {
-              for (int j = 0; j < 16; ++j)
-                if (n0 + 2 * j < p.N) *reinterpret_cast<uint32_t*>(crow + c * 32 + 2 * j) = o[j];
+              store4(crow + n, pack_bf16x2(x0, x1), p.hints & 4);
             }
           }
         }
       }
-      // all of this warp's tcgen05.ld have completed (wait::ld above) -> hand the accumulator stage back
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -319,9 +231,8 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParam
   if (!CONV) p.num_m = (p.M + BM - 1) / BM;  // CONV: set by the caller (images x tiles per image)
   p.num_n = (p.N + BN - 1) / BN;
   p.num_tiles = p.num_m * p.num_n;
-  // Raster group: group_m M-tiles share one sweep over the N tiles. Measured on B200 at M=65568 (A/B in one process
-  // per value, profiles/r01_gemm_group_ab.txt): wide outputs (148 N-tiles, gate|up) are fastest at 16, narrow ones
-  // (14-18 N-tiles: qkv, o_proj, down_proj) at 32; 8 and 64 lose 5-15 % either way.
+  // Raster group: group_m M-tiles share one sweep over the N tiles: 16 for wide outputs (gate|up: 148 N-tiles), 32 for
+  // narrow ones (14-18 N-tiles: qkv, o_proj, down_proj).
   {
     static const int env_g = [] { const char* e = getenv("BAGEL_GEMM_GROUP_M"); return e ? atoi(e) : 0; }();
     static const int env_n = [] { const char* e = getenv("BAGEL_GEMM_GROUP_N"); return e ? atoi(e) : -1; }();
@@ -368,7 +279,7 @@ extern "C" int bagel_gemm_bf16(const void* A, long long lda, const void* W, long
     return set_error(BAGEL_ERR_ALIGN, "bagel_gemm_bf16: pointers must be 16-byte aligned");
   if ((epilogue == EPI_RESID || epilogue == EPI_RESID_F32) && (resid == nullptr || (ldr % 8)))
     return set_error(BAGEL_ERR_ARG, "bagel_gemm_bf16: the residual epilogues need resid with ldr %% 8 == 0");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
 
   GemmParams p{};
   p.M = M; p.N = N; p.K = K;
@@ -388,14 +299,6 @@ extern "C" int bagel_gemm_bf16(const void* A, long long lda, const void* W, long
   static const bool skinny_on = [] { const char* e = getenv("BAGEL_GEMM_SKINNY"); return !(e && atoi(e) == 0); }();
   if (skinny_on && gemm_skinny_supported(M, N, K, epilogue))
     return gemm_skinny(A, lda, W, ldw, C, ldc, M, N, K, bias, resid, ldr, row_map, epilogue, s);
-
-  // the large projections: 256 x 256 tiles on CTA pairs (tcgen05 cta_group::2), gemm2.cu
-  if (gemm2_supported(M, N, K, epilogue)) {
-    CUtensorMap tmA2, tmB2;
-    if (int rc = make_tmap_2d_bf16(&tmA2, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM)) return rc;
-    if (int rc = make_tmap_2d_bf16(&tmB2, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, 128)) return rc;
-    return gemm2_launch(tmA2, tmB2, p, epilogue, s);
-  }
 
   int bn;
   if (epilogue == EPI_SWIGLU) {
@@ -436,7 +339,7 @@ extern "C" int bagel_conv2d_nhwc_bf16(const void* x, int B, int Hi, int Wi, int 
   if (B <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0) return set_error(BAGEL_ERR_SHAPE, "bagel_conv2d_nhwc_bf16: bad sizes");
   if (((uintptr_t)x | (uintptr_t)w | (uintptr_t)out | (uintptr_t)bias | (uintptr_t)resid) & 15)
     return set_error(BAGEL_ERR_ALIGN, "bagel_conv2d_nhwc_bf16: pointers must be 16-byte aligned");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
 
   GemmParams p{};
   p.Ho = Ho; p.Wo = Wo;
@@ -484,7 +387,7 @@ extern "C" int bagel_gemm_qkv_norm_rope(const void* A, long long lda, const void
     return set_error(BAGEL_ERR_ALIGN, "bagel_gemm_qkv_norm_rope: K and leading dims must be multiples of 8");
   if (bias == nullptr || q_w0 == nullptr || k_w0 == nullptr || cos_t == nullptr || sin_t == nullptr)
     return set_error(BAGEL_ERR_ARG, "bagel_gemm_qkv_norm_rope: bias, norm weights and RoPE tables are required");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   GemmParams p{};
   p.M = M; p.N = N; p.K = K;
   p.bias = static_cast<const __nv_bfloat16*>(bias);
@@ -499,11 +402,6 @@ extern "C" int bagel_gemm_qkv_norm_rope(const void* A, long long lda, const void
   p.qkv.Hq = Hq; p.qkv.Hk = Hk; p.qkv.eps = eps; p.qkv.fp32_flow = fp32_flow;
   CUtensorMap tmA, tmB;
   if (int rc = make_tmap_2d_bf16(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM)) return rc;
-  // the large calls (all rows of a denoising step): CTA-pair kernel, each CTA stages half of the 256-row W tile (gemm2.cu)
-  if (gemm2_supported(M, N, K, EPI_QKV)) {
-    if (int rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, 128)) return rc;
-    return gemm2_launch(tmA, tmB, p, EPI_QKV, static_cast<cudaStream_t>(stream));
-  }
   if (int rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, 256)) return rc;
   return launch_gemm<256, EPI_QKV>(tmA, tmB, p, static_cast<cudaStream_t>(stream));
 }

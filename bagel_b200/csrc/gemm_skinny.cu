@@ -1,14 +1,15 @@
 // Skinny-M GEMM for the token-by-token decode path (and the few und-expert rows of a MoT layer):
 //   C[M, N] = epilogue(A[M, K] * W[N, K]^T),  M <= 64.
 // With M this small the GEMM is a pure weight stream (HBM bound: 2*N*K bytes), so the tile is built around W:
-//   * operands are SWAPPED: a 128-row slab of W is the tcgen05 "A" operand (M=128), the (padded) tokens are the
+//   * operands are SWAPPED: a 128-row slab of W is the wgmma "A" operand (two m64 halves), the (padded) tokens are the
 //     "B" operand (N = MT in {16, 32, 64}). Of every pipeline stage's bytes 80-94 % are weights; the regular
 //     kernel's 128-token tile would spend 80 % of its shared-memory fill on zero padding.
 //   * split-K over a thread-block CLUSTER: when N/128 tiles cannot fill the GPU the K range is divided over up to 8
 //     CTAs of one cluster; partial accumulators are exchanged through distributed shared memory and summed by the
 //     cluster's rank-0 CTA in rank order (deterministic, no atomics, no workspace).
-//   * accumulator in TMEM is [128 features x MT tokens]: an epilogue thread owns one output feature, so bias is a
-//     scalar and every store instruction of a warp writes 32 consecutive features of one token (64 B).
+//   * the accumulator [128 features x MT tokens] is parked in shared memory (over the drained operand ring); an epilogue
+//     thread owns one output feature, so bias is a scalar and every store instruction of a warp writes 32 consecutive
+//     features of one token (64 B).
 // Epilogue rounding points are the ones of gemm.cu (the reference's autocast casts).
 #include "common.cuh"
 #include "host_util.h"
@@ -18,7 +19,7 @@ namespace bagel {
 
 namespace {
 
-constexpr int kThreads = 192;   // warp0 TMA, warp1 MMA (+TMEM alloc), warps 2-5 epilogue
+constexpr int kThreads = 256;   // warpgroup 0: TMA (warp 0); warpgroup 1: wgmma + epilogue
 constexpr int kBK = 64;         // K elements per pipeline stage (one 128 B swizzle atom)
 constexpr int kMaxStages = 12;
 
@@ -36,7 +37,6 @@ struct SkinnyParams {
   int split;    // cluster size along K
   int num_k;    // K blocks in total
   int stages;
-  uint32_t tmem_cols;
 };
 
 __device__ __forceinline__ float gelu_tanh_s(float x) {
@@ -45,15 +45,6 @@ __device__ __forceinline__ float gelu_tanh_s(float x) {
 }
 __device__ __forceinline__ float silu_s(float x) { return x / (1.0f + __expf(-x)); }
 
-__device__ __forceinline__ void tmem_alloc_n(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_n(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -70,24 +61,23 @@ __device__ __forceinline__ float ld_dsmem_f32(uint32_t local_addr, uint32_t rank
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
   return v;
 }
+// the 128 threads of the MMA warpgroup only
+__device__ __forceinline__ void mma_wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 // NW = 128-row W slabs per CTA (2 only for SwiGLU: the gate slab and the matching up slab of the interleaved weight).
-template <int NW, int EPI>
-__global__ void __launch_bounds__(kThreads, 2)
+template <int NW, int EPI, int MT>
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmA,
                    const SkinnyParams p) {
   static_assert((EPI == S_SWIGLU) == (NW == 2), "two W slabs exactly for SwiGLU");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int kWBytes = NW * 128 * kBK * 2;
-  const int a_bytes = p.MT * kBK * 2;
-  const int stage_bytes = kWBytes + a_bytes;
+  constexpr int stage_bytes = kWBytes + MT * kBK * 2;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kMaxStages;
-  uint64_t* tfull_bar = bars + 2 * kMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull_bar + 1);
-  float* part = reinterpret_cast<float*>(smem);  // split-K partials alias the (drained) operand ring
+  float* part = reinterpret_cast<float*>(smem);  // [NW * MT tokens][128 features] accumulators, over the drained ring
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -96,21 +86,16 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   const int kb_begin = (int)(((long long)rank * p.num_k) / p.split);
   const int kb_end = (int)(((long long)(rank + 1) * p.num_k) / p.split);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmW);
     tma_prefetch_desc(&tmA);
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);   // one arrive per MMA warp
     }
-    mbar_init(tfull_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc_n(tmem_slot, p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   pdl_launch_dependents();   // the next PDL kernel may start its own weight prefetch while this one streams
 
@@ -138,54 +123,66 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (elect_one_lane()) {   // not `lane == 0`: see common.cuh
-      const uint32_t idesc = umma_idesc_bf16(128, (uint32_t)p.MT, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t st = smem_u32(smem + stage * stage_bytes);
-        const uint64_t b_desc = umma_desc_kmajor_sw128(st + kWBytes);
+  } else if (warp >= 4) {
+    // MMA warpgroup: acc[w][half] = W slab w, rows [64 half, 64 half + 64) x MT tokens
+    float acc[NW][2][MT / 2];
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t st = smem_u32(smem + stage * stage_bytes);
+      const uint64_t b_desc = gmma_desc_kmajor_sw128(st + kWBytes);
+      wgmma_fence();
 #pragma unroll
-        for (int w = 0; w < NW; ++w) {
-          const uint64_t a_desc = umma_desc_kmajor_sw128(st + w * (128 * kBK * 2));
+      for (int w = 0; w < NW; ++w) {
 #pragma unroll
-          for (int k = 0; k < kBK / 16; ++k)
-            umma_ss(tmem_base + w * p.MT, a_desc + 2 * k, b_desc + 2 * k, idesc, (kb > kb_begin) || (k > 0));
+        for (int hf = 0; hf < 2; ++hf) {
+          const uint64_t a_desc = gmma_desc_kmajor_sw128(st + w * (128 * kBK * 2) + hf * (64 * kBK * 2));
+#pragma unroll
+          for (int k = 0; k < kBK / 16; ++k) wgmma_ss<MT>(acc[w][hf], a_desc + 2 * k, b_desc + 2 * k, (kb > kb_begin) || (k > 0));
         }
-        umma_commit(&empty_bar[stage]);
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
-      umma_commit(tfull_bar);
+      wgmma_commit();
+      if (kb > kb_begin) {
+        wgmma_wait<1>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
-    __syncwarp();
-  } else {
-    // epilogue warps: wait for this CTA's accumulator; non-leader CTAs of a split park it in shared memory
-    pdl_wait();   // residual reads / output writes below must follow the predecessor kernel
-    mbar_wait(tfull_bar, 0);
-    tc_fence_after();
-    if (p.split > 1 && rank != 0) {
-      const int quarter = warp & 3;
-      const int r = quarter * 32 + lane;
-      const uint32_t t_acc = tmem_base + (uint32_t(quarter * 32) << 16);
-      for (int c = 0; c < p.MT; c += 16) {
-        uint32_t v[16];
-        tmem_ld_x16(t_acc + c, v);
-        tmem_ld_wait();
+    wgmma_wait<0>();
 #pragma unroll
-        for (int j = 0; j < 16; ++j) part[(c + j) * 128 + r] = __uint_as_float(v[j]);
-      }
+    for (int w = 0; w < NW; ++w)
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) gmma_fence_operand(acc[w][hf]);
+    mma_wg_sync();   // every warp's wgmma has retired: the operand ring may be overwritten
+    const int wq = warp & 3;
+    if (kb_end > kb_begin) {
+#pragma unroll
+      for (int w = 0; w < NW; ++w)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+          for (int c = 0; c < MT / 8; ++c)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int r = hf * 64 + wq * 16 + (lane >> 2) + 8 * (i >> 1);    // feature within the slab
+              const int m = 8 * c + 2 * (lane & 3) + (i & 1);                  // token
+              part[(w * MT + m) * 128 + r] = acc[w][hf][4 * c + i];
+            }
+    } else {   // empty K range (split > num_k cannot happen, but keep the contract): contributes zeros
+      for (int i = threadIdx.x - 128; i < NW * MT * 128; i += 128) part[i] = 0.f;
     }
   }
 
-  if (p.split > 1) cluster_sync_all();   // partials visible cluster-wide
+  // partials visible CTA-wide (and, with a split, cluster-wide)
+  if (p.split > 1) cluster_sync_all();
+  else __syncthreads();
 
-  if (warp >= 2 && rank == 0) {
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t t_acc = tmem_base + (uint32_t(quarter * 32) << 16);
+  if (warp >= 4 && rank == 0) {
+    pdl_wait();   // residual reads / output writes below must follow the predecessor kernel
+    const int r = threadIdx.x - 128;
     const int n_out = (EPI == S_SWIGLU) ? p.N / 2 : p.N;
     const int n = tile * 128 + r;            // output feature owned by this thread
     const bool n_ok = n < n_out;
@@ -193,11 +190,14 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
     if (EPI != S_SWIGLU && p.bias != nullptr && n_ok) bias = __bfloat162float(p.bias[n]);
     const uint32_t part_addr = smem_u32(part + r);
     for (int c = 0; c < p.M; c += 16) {
-      uint32_t v[16], u[16];
-      tmem_ld_x16(t_acc + c, v);
-      if constexpr (EPI == S_SWIGLU) tmem_ld_x16(t_acc + p.MT + c, u);
+      float v[16], u[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        v[j] = part[(c + j) * 128 + r];
+        if constexpr (EPI == S_SWIGLU) u[j] = part[(MT + c + j) * 128 + r];
+      }
       // Output rows and residual values of this chunk: every load is issued here, before the first dependent store (a
-      // load -> store -> load chain per token cost one L2 round trip per token: 16 us of a 24 us o_proj at 32 tokens).
+      // load -> store -> load chain per token costs one L2 round trip per token).
       long long orow[16];
       float rv[16];
 #pragma unroll
@@ -210,12 +210,10 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
         for (int j = 0; j < 16; ++j)
           rv[j] = (n_ok && c + j < p.M) ? __bfloat162float(p.resid[orow[j] * p.ldr + n]) : 0.f;
       }
-      tmem_ld_wait();
       if constexpr (NW == 1) {
         for (uint32_t pr = 1; pr < (uint32_t)p.split; ++pr) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
-            v[j] = __float_as_uint(__uint_as_float(v[j]) + ld_dsmem_f32(part_addr + (uint32_t)((c + j) * 128 * 4), pr));
+          for (int j = 0; j < 16; ++j) v[j] += ld_dsmem_f32(part_addr + (uint32_t)((c + j) * 128 * 4), pr);
         }
       }
       if (n_ok) {
@@ -223,7 +221,7 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
         for (int j = 0; j < 16; ++j) {
           const int m = c + j;
           if (m < p.M) {
-            float x = __uint_as_float(v[j]) + bias;
+            float x = v[j] + bias;
             if constexpr (EPI == S_RESID) {
               x = rv[j] + bf16_round(x);
             } else if constexpr (EPI == S_GELU) {
@@ -231,7 +229,7 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
             } else if constexpr (EPI == S_SILU) {
               x = silu_s(bf16_round(x));
             } else if constexpr (EPI == S_SWIGLU) {
-              x = bf16_round(silu_s(bf16_round(__uint_as_float(v[j])))) * bf16_round(__uint_as_float(u[j]));
+              x = bf16_round(silu_s(bf16_round(v[j]))) * bf16_round(u[j]);
             }
             p.C[orow[j] * p.ldc + n] = __float2bfloat16_rn(x);
           }
@@ -241,18 +239,12 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   }
 
   if (p.split > 1) cluster_sync_all();   // peers stay resident until rank 0 has read their partials
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_n(tmem_base, p.tmem_cols);
-  }
 }
 
-template <int NW, int EPI>
-int launch(const CUtensorMap& tmW, const CUtensorMap& tmA, const SkinnyParams& p, int tiles, int smem_bytes,
+template <int NW, int EPI, int MT>
+int launch_mt(const CUtensorMap& tmW, const CUtensorMap& tmA, const SkinnyParams& p, int tiles, int smem_bytes,
            cudaStream_t stream) {
-  auto kern = gemm_skinny_kernel<NW, EPI>;
+  auto kern = gemm_skinny_kernel<NW, EPI, MT>;
   static int attr_bytes = 0;
   if (smem_bytes > attr_bytes) {
     BAGEL_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -278,6 +270,14 @@ int launch(const CUtensorMap& tmW, const CUtensorMap& tmA, const SkinnyParams& p
   BAGEL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmW, tmA, p));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return 0;
+}
+
+template <int NW, int EPI>
+int launch(const CUtensorMap& tmW, const CUtensorMap& tmA, const SkinnyParams& p, int tiles, int smem_bytes,
+           cudaStream_t stream) {
+  if (p.MT == 16) return launch_mt<NW, EPI, 16>(tmW, tmA, p, tiles, smem_bytes, stream);
+  if (p.MT == 32) return launch_mt<NW, EPI, 32>(tmW, tmA, p, tiles, smem_bytes, stream);
+  return launch_mt<NW, EPI, 64>(tmW, tmA, p, tiles, smem_bytes, stream);
 }
 
 }  // namespace
@@ -308,9 +308,8 @@ int gemm_skinny(const void* A, long long lda, const void* W, long long ldw, void
   // portable cluster sizes only (<= 8): larger ones need cudaFuncAttributeNonPortableClusterSizeAllowed and fail at launch
   static const int env_split = [] { const char* e = getenv("BAGEL_SKINNY_SPLIT"); const int v = e ? atoi(e) : 0; return v > 8 ? 8 : v; }();
   static const int env_stages = [] { const char* e = getenv("BAGEL_SKINNY_STAGES"); return e ? atoi(e) : 0; }();
-  // Measured on B200 at B=32 (profiles/r01_skinny_gemm_split_stage_sweep.txt): what matters is (a) >= ~12 K blocks
-  // per CTA, (b) about 1.5 CTAs per SM in total and (c) SMALL shared memory per CTA — a cluster whose CTAs each need a
-  // whole SM (deep ring) often cannot be placed in one GPC and the grid runs in two waves (61 vs 34 us on down_proj).
+  // What matters: (a) >= ~12 K blocks per CTA, (b) about 1.5 CTAs per SM in total and (c) SMALL shared memory per CTA — a
+  // cluster whose CTAs each need a whole SM (deep ring) may not be placeable in one GPC, and the grid then runs in two waves.
   int split = 1;
   if (nw == 1) {
     if (env_split > 0) split = env_split;
@@ -335,12 +334,10 @@ int gemm_skinny(const void* A, long long lda, const void* W, long long ldw, void
   if (stages < 2) stages = 2;
   const int per_cta_k = (p.num_k + split - 1) / split;
   if (stages > per_cta_k) stages = per_cta_k < 2 ? 2 : per_cta_k;
-  if (split > 1 && stages * stage_bytes < 128 * p.MT * 4) stages = (128 * p.MT * 4 + stage_bytes - 1) / stage_bytes;
+  // the accumulators [nw * MT][128] fp32 are parked over the ring
+  if (stages * stage_bytes < nw * 128 * p.MT * 4) stages = (nw * 128 * p.MT * 4 + stage_bytes - 1) / stage_bytes;
   p.stages = stages;
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(nw * p.MT)) cols *= 2;
-  p.tmem_cols = cols;
-  const int smem_bytes = stages * stage_bytes + 1024 + (2 * kMaxStages + 2) * 8;
+  const int smem_bytes = stages * stage_bytes + 1024 + 2 * kMaxStages * 8;
 
   CUtensorMap tmW, tmA;
   if (int rc = make_tmap_2d_bf16(&tmW, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, kBK, nw * 128)) return rc;

@@ -15,7 +15,7 @@ namespace bagel {
 extern std::atomic<long long> g_launches;       // kernels launched by this library (bagel_launch_count)
 int set_error(int code, const char* fmt, ...);  // records thread-local message, returns `code`
 int sm_count();                                 // SMs of the current device (cached per device)
-int require_sm100();                            // 0 if current device is sm_100, else BAGEL_ERR_ARCH
+int require_sm90();                             // 0 if current device is sm_90, else BAGEL_ERR_ARCH
 // 2D bf16 tensor map: global [rows, cols] with row pitch `ld` elements; box [box_rows, box_cols];
 // 128-byte swizzle; out-of-bounds reads are zero-filled.
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t ld,

@@ -1,6 +1,6 @@
 // HBM-bound kernels of the FLUX VAE (modeling/autoencoder.py): GroupNorm(32)+swish on NHWC activations,
 // nearest 2x upsampling, row softmax for the single-head d=512 mid attention, bf16 transpose.
-// The convolutions themselves are the implicit-GEMM tcgen05 kernel in gemm.cu (bagel_conv2d_nhwc_bf16).
+// The convolutions themselves are the implicit-GEMM wgmma kernel in gemm.cu (bagel_conv2d_nhwc_bf16).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -15,7 +15,7 @@ namespace bagel {
 // x: [B, HW, C] bf16 (NHWC), G groups of C/G consecutive channels. Deterministic: no atomics, the slabs are
 // reduced in a fixed order by pass 2. HBM-bound: the grid is sized so that every SM holds several CTAs and every
 // thread keeps four 16-byte loads in flight (round 1 launched 64 CTAs with one load per thread in flight per image:
-// 0.24 TB/s at 1024^2 x 128 channels, a third of the whole VAE decode — profiles/r02_vae_decode_launches.csv).
+// 0.24 TB/s at 1024^2 x 128 channels, a third of the whole VAE decode).
 // ---------------------------------------------------------------------------------------------
 constexpr int kGnMaxSlabs = 1024;
 

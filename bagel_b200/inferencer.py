@@ -4,7 +4,7 @@ Same class, methods, keyword arguments and defaults as the reference's inference
 maintained (main / cfg_text / cfg_img), each a dict {kv_lens, ropes, past_key_values}; contexts are deep-copied at
 the same points as the reference so the CFG branches see the same prefixes.
 
-Scope (SURVEY.md §8): the text->image and text-decode paths run on the B200 kernels. Image *inputs* need the
+Scope (SURVEY.md §8): the text->image and text-decode paths run on the H100 kernels. Image *inputs* need the
 SigLIP encoder / VAE encoder (`update_context_image`) and decoded image *outputs* need the VAE decoder
 (`decode_image`); both delegate to the `vit_model` / `vae_model` objects handed to the constructor and raise if
 those are absent.

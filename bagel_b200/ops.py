@@ -1,5 +1,5 @@
 """torch.Tensor-facing wrappers over the C ABI (include/bagel_b200.h). PyTorch is used only for device
-memory and streams; every call below lands in a hand-written sm_100a kernel or raises."""
+memory and streams; every call below lands in a hand-written sm_90a kernel or raises."""
 from __future__ import annotations
 
 import ctypes as C

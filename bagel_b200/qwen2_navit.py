@@ -3,7 +3,7 @@
 Mirrors the inference API of the reference's modeling/bagel/qwen2_navit.py (NaiveCache :207-221,
 Qwen2Model.forward_inference :1018-1092, Qwen2ForCausalLM.forward_inference :1157-1188, and the MoT layer /
 attention they call :499-600, :757-831) with the same argument names and meaning, but executes every layer as a
-fixed sequence of hand-written sm_100a kernels (bagel_b200.ops). There is no nn.Module / autograd here: weights
+fixed sequence of hand-written sm_90a kernels (bagel_b200.ops). There is no nn.Module / autograd here: weights
 are plain device tensors in fused layouts (QKV concatenated, gate/up interleaved for the SwiGLU epilogue).
 
 Numerics: `dtype_mode="A"` (default) follows the reference with bf16 weights under autocast (app.py:111 +

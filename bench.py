@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — BAGEL-7B-MoT text->image denoising throughput on B200 (BASELINE.json metric).
+"""bench.py — BAGEL-7B-MoT text->image denoising throughput on H100 (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 Workload (BASELINE.json configs[1], SURVEY.md §8d cfg 2): BAGEL-7B-MoT random-init, 1024x1024 (4096 latent tokens
@@ -12,14 +12,16 @@ A "step" is ONE denoising step of the whole batch: latent-in -> 28 MoT layers ov
 -> CFG + renorm + Euler update (every step costs the same, 49 of them make one image batch). Reported:
   value   images/s (whole job, all GPUs) = global_batch / (49 * s_per_step); x_t and all inputs resident in HBM,
           W warm-up steps, exactly K timed steps, CUDA events, max over ranks. The activations + weights touched
-          per step (> 30 GB) far exceed the 126 MB L2, so no explicit L2 flush is needed (config.l2: "working set").
+          per step (> 30 GB) far exceed the 50 MB L2, so no explicit L2 flush is needed (config.l2: "working set").
   e2e     the same metric through the public API: Bagel.generate_image(**prepare_vae_latent(...)) from host
           (pinned) init noise to host latents, including planning, H2D/D2H, and for N > 1 the NCCL all-gather of
           the final latents.
-  roofline   the dominant kernel (SwiGLU gate/up GEMM, tcgen05): algorithmic FLOPs / CUDA-event time per launch.
+  roofline   the dominant kernel (SwiGLU gate/up GEMM, wgmma): algorithmic FLOPs / CUDA-event time per launch.
   cpu_baseline  the oracle (CPU port of the reference path) on this box's host cores, bounded sample.
 --impl reference times the reference's CPU path (the oracle port: the Python reference cannot travel to the
 box) with all host threads on a bounded sample of the same workload and prints the same JSON shape.
+--dump-outputs DIR writes the latents x_t after the last timed step ([batch, 4096, 64] fp32, rank 0) as DIR/latents.npy.
+All inputs and weights come from fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -59,7 +61,12 @@ def parse_args():
                          "gpu_library_baseline, parity, strong_scaling)")
     ap.add_argument("--blocks", default="attn,und,edit,library,strong",
                     help="comma list of extra blocks to run (default: all)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the latents after the last timed step to DIR/latents.npy (float32)")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    return args
 
 
 def measured_peaks():
@@ -68,11 +75,12 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; not measured, and not reached
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback (H100 SXM data sheet)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -333,6 +341,11 @@ def main():
     torch.cuda.synchronize()
     launches = _cabi.launch_count() - l0
     swiglu_ms = ops.kernel_timer_stop()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        lat = torch.stack(runner.latents(), 0).float().cpu().numpy()     # [B, 4096, 64]: x_t after the last timed step
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), lat)
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
@@ -350,34 +363,20 @@ def main():
     rows = 2 * B * ((args.image_size // 16) ** 2 + 2)  # both CFG branches in one packed call
     flops_launch = 2.0 * rows * (2 * cfg.intermediate_size) * cfg.hidden_size
     roof = None
-    traffic, traffic_src = None, None
-    prof = os.path.join(ROOT, "profiles", "r02_gemm2_swiglu_ncu_full.csv")
-    if os.path.exists(prof) and rows == 65568:   # the capture was taken on exactly this launch shape
-        try:
-            vals = {}
-            for ln in open(prof):
-                if ln.startswith('"dram__bytes_read.sum",') or ln.startswith('"dram__bytes_write.sum",'):
-                    name, unit, v = [x.strip().strip('"') for x in ln.split(",")]
-                    vals[name] = float(v) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[unit]
-            traffic = vals["dram__bytes_read.sum"] + vals["dram__bytes_write.sum"]
-            traffic_src = "profiles/r02_gemm2_swiglu_ncu_full.csv (ncu --set full, one launch of this kernel/shape, this build)"
-        except Exception:
-            traffic = None
     if swiglu_ms:
         avg_ms = statistics.mean(swiglu_ms)
         ach = flops_launch / (avg_ms * 1e-3) / 1e12
         peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops")))
-        roof = {"kernel": "gemm2_bf16_kernel<SWIGLU> (CTA-pair tcgen05 cta_group::2; gate|up projection + SiLU*up epilogue)",
+        roof = {"kernel": "gemm_bf16_kernel<256, SWIGLU> (wgmma; gate|up projection + SiLU*up epilogue)",
                 "bound": "tensor",
-                "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic,
-                "traffic_unit": "bytes/launch (dram read+write)", "traffic_source": traffic_src,
+                "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
                 "algorithmic_bytes_per_launch": 2.0 * (rows * cfg.hidden_size + 2 * cfg.intermediate_size * cfg.hidden_size
                                                        + rows * cfg.intermediate_size),
                 "peak_source": f"{peak_src} bf16_tflops_sustained (kernel timed inside a long step)",
                 "launches_timed": len(swiglu_ms), "avg_launch_ms": avg_ms,
                 "flops_per_launch": flops_launch}
     model_flops_img = 98 * (4098 * 13.05e9 + 4 * 4098 * (4098 + 66) * 3584 * 28)  # SURVEY.md §6
-    mfu = value / world * model_flops_img / (float(peaks.get("bf16_tflops_sustained", 1400.0)) * 1e12)
+    mfu = value / world * model_flops_img / (float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops"))) * 1e12)
 
     # ---------------- end to end through the public API ----------------
     e2e = None
@@ -497,7 +496,7 @@ def main():
                 extra["und_prefill"] = extra["edit"] = r
                 need_vit = False
         if need_vit and world == 1 and "und" in blocks:
-            extra.update(guarded("und", lambda: bb.und_prefill_and_decode_block(model, dev)))
+            extra.update(guarded("und", lambda: bb.und_prefill_and_decode_block(model, dev, hbm_gbs=float(peaks["hbm_gbs"]))))
             torch.cuda.empty_cache()
         if need_vit and "edit" in blocks:
             def edit():
@@ -537,7 +536,7 @@ def main():
                                    "denoising step of the batch; images/s = global_batch/(49*s_per_step)",
                        "model": "BAGEL-7B-MoT (random init)", "global_batch": B * world, "per_gpu_batch": B,
                        "image_size": args.image_size, "layers": cfg.num_hidden_layers,
-                       "parallelism": f"replica-dp{world}", "l2": "working set per step >> 126 MB L2 (no flush needed)"},
+                       "parallelism": f"replica-dp{world}", "l2": "working set per step >> 50 MB L2 (no flush needed)"},
             "per_gpu_images_per_s": value / world, "mfu_vs_sustained_peak": mfu,
             "roofline": roof, "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks,
             "e2e_taylorseer": e2e_ts,

@@ -1,4 +1,4 @@
-/* bagel_b200 — C ABI of the B200-native (sm_100a) kernels behind BAGEL's inference forward path.
+/* bagel_b200 — C ABI of the H100-native (sm_90a) kernels behind BAGEL's inference forward path.
  *
  * The reference (ByteDance-Seed/Bagel) is pure Python; the only native seam it has is
  * `flash_attn_varlen_func` (modeling/bagel/qwen2_navit.py:361,579; modeling/bagel/siglip_navit.py:232).
@@ -46,7 +46,7 @@ long long bagel_launch_count(void);
 #define BAGEL_EPI_RESID_F32 7 /* C (fp32) = resid (fp32 [*, ldr]) + bf16(acc + bias)    fp32 residual stream: dtype mode B
                               * (fp32 master weights under autocast, eval/gen/gen_images_mp.py:159-175, :73)            */
 
-/* C[M,N] = epilogue(A[M,K] @ W[N,K]^T), bf16 in / fp32 accumulate (tcgen05, TMEM) / bf16 out.
+/* C[M,N] = epilogue(A[M,K] @ W[N,K]^T), bf16 in / fp32 accumulate (wgmma) / bf16 out.
  * Replaces nn.Linear at modeling/bagel/qwen2_navit.py:515-517,529-536 (q/k/v_proj{,_moe_gen}),
  * :589-594 (o_proj{,_moe_gen}), modeling/qwen2/modeling_qwen2.py:200-201 (gate/up/down_proj),
  * modeling/bagel/bagel.py:803,832 (vae2llm, llm2vae), modeling/bagel/modeling_utils.py:84-110,120-124.
@@ -153,7 +153,7 @@ int bagel_cfg_euler_step(const void* v, const void* v_text, const void* v_img, l
 /* y[i] = bf16(x[i]) — the autocast cast in front of vae2llm (modeling/bagel/bagel.py:803). */
 int bagel_cast_f32_to_bf16(const float* x, void* y, long long n, void* stream);
 
-/* 2-D convolution on NHWC bf16 activations as an im2col-free implicit GEMM on tcgen05 (FLUX VAE convs:
+/* 2-D convolution on NHWC bf16 activations as an im2col-free implicit GEMM on wgmma (FLUX VAE convs:
  * modeling/autoencoder.py:76-80 ResnetBlock, :102-108 Downsample (stride 2, pad right/bottom), :114-119 Upsample conv,
  * :43-48 AttnBlock 1x1, :139,170,221,248 conv_in/conv_out — cuDNN NCHW convolutions in the reference).
  *   x [B, Hi, Wi, Cin], w [Cout, ksize, ksize, Cin] (reference layout [Cout, Cin, kh, kw] permuted once at load),

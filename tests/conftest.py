@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100: pytest -m gpu)")
     # A/B builds (tools/build_variant.py): run the SAME tests against a variant library. Test infrastructure only — the
     # package itself always loads bagel_b200/libbagel_b200.so.
     lib = os.environ.get("BAGEL_TEST_LIB")

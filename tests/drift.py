@@ -1,6 +1,6 @@
 """Shared by tests/test_gpu_drift_7b.py and tools/gpu_drift_7b.py: run the SAME text->image denoising job through
 
-  product  bagel_b200 (C ABI -> sm_100a kernels)
+  product  bagel_b200 (C ABI -> sm_90a kernels)
   fa2      the oracle on cuda with flash_attn_varlen_func  = the reference as it executes on a GPU
   sdpa     the oracle on cuda with its fp32 per-sample SDPA = the reference as pinned on the CPU (attention shim)
   truth    the oracle in fp32 end to end on the same bf16-valued weights (optional, first `truth_steps` steps)
@@ -59,11 +59,21 @@ def run(layers: int = 28, evals: int = 49, truth_steps: int = 0, batch: int = 1,
     torch.cuda.synchronize()
     out["t"]["product"] = time.perf_counter() - t0
     out["x"]["product"] = xs
-    del runner
+    del runner, ctx
     log(f"product: {len(xs)} steps in {out['t']['product']:.1f} s")
 
     # ---- reference legs on the same weights ----
+    # The legs own the weights from here on: the product's activation workspaces go before the export, its interleaved
+    # gate|up weights (de-interleaved copies are in `sd`) right after it, so the 7B job holds one copy of the weights.
+    lm = model.language_model.model
+    lm._ws.clear()
+    torch.cuda.empty_cache()
     sd = gpu_leg.export_reference_state_dict(model)
+    for layer in lm.layers:
+        for e in (layer.und, layer.gen):
+            if e is not None:
+                e.wgu = None
+    torch.cuda.empty_cache()
     fc = gpu_leg.flow_config(model)
     tok = synthetic.RandomIdTokenizer(1)
     prompt_ids = [tok.encode("64") for _ in range(batch)]
@@ -92,7 +102,7 @@ def run(layers: int = 28, evals: int = 49, truth_steps: int = 0, batch: int = 1,
 
 
 def report(res: Dict, every: int = 1) -> str:
-    """Text table of the per-step distances (profiles/r02_drift_7b.txt)."""
+    """Text table of the per-step distances."""
     x = res["x"]
     lines = []
     pairs = [("product", "fa2"), ("sdpa", "fa2"), ("product", "sdpa")]

@@ -10,7 +10,7 @@ from bagel_b200 import _cabi, build, ops
 
 @pytest.fixture(scope="module")
 def lib():
-    build.build()  # no-op when fresh; cross-compiles sm_100a without a GPU
+    build.build()  # no-op when fresh; cross-compiles sm_90a without a GPU
     return _cabi.lib()
 
 

@@ -1,4 +1,4 @@
-"""-m gpu: adversarial inputs for the tcgen05 attention kernel's LAZY RESCALING path (bagel_b200/csrc/attn.cu: scores are
+"""-m gpu: adversarial inputs for the attention kernel's LAZY RESCALING path (bagel_b200/csrc/attn.cu: scores are
 exponentiated against a reference maximum carried over from earlier key blocks; a block is redone exactly only when its
 row sum leaves [0, 2^30]) and the large / causal shapes of BASELINE configs[4] (L = 4k causal, 16k), which the N(0,1)
 tests in test_gpu_kernels.py never stress: row maxima that grow with every key block, |logit| up to ~100 (what trained

@@ -2,7 +2,7 @@
 evaluations, text CFG scale 2, one 1024^2 sample — product vs the reference-equivalent GPU legs (tests/drift.py,
 oracle/gpu_leg.py). The tolerance is derived from the MEASURED noise floor of the reference itself (oracle+flash-attn
 vs oracle+fp32-SDPA on identical inputs: two valid executions of the reference that differ only in the attention
-kernel's internal rounding), not chosen by the builder; profiles/r02_drift_7b.txt holds the per-step table of the
+kernel's internal rounding), not chosen by the builder; tools/gpu_drift_7b.py prints the per-step table of the
 same run including the fp32 truth for all 49 steps. north_star's "1e-3 rtol" is compared against that floor in DESIGN.md §4."""
 import pytest
 import torch
@@ -14,14 +14,15 @@ pytestmark = pytest.mark.gpu
 # product-vs-reference distance allowed, in units of the reference's own fa2-vs-sdpa distance at the same step. The
 # product differs from either leg in MORE places than the legs differ from each other (GEMM accumulation order and
 # fused-epilogue rounding on top of the attention kernel), so a factor somewhat above 1 is the expectation for "just
-# another bf16 execution of the same network"; measured 28-layer/49-step values are in profiles/r02_drift_7b.txt.
+# another bf16 execution of the same network".
 FLOOR_FACTOR = 3.0
 
 
 @pytest.fixture(scope="module")
 def res():
-    if torch.cuda.get_device_properties(0).total_memory < 100e9:
-        pytest.skip("needs the 7B weights twice (product layouts + de-interleaved gate/up) in HBM")
+    if torch.cuda.get_device_properties(0).total_memory < 64e9:
+        # peak 44 GB allocated (48 GB reserved) on an H100 80GB: 7B weights + the reference layout of gate/up + activations
+        pytest.skip("needs about 48 GB of device memory")
     return drift.run(layers=28, evals=49, truth_steps=2, batch=1, image_size=1024, log=lambda *a: None)
 
 

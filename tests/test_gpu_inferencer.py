@@ -48,7 +48,7 @@ def _check_image(name, img, ref):
     d = np.abs(got - ref)
     print(f"{name}: |d| mean {d.mean():.2f} levels, p99 {np.percentile(d, 99):.0f}, max {d.max()}")
     # random-init VAE decoder output is noise-like (std ~67 levels): a wrong context / branch / seed gives |d| ~ 75
-    # measured on B200: mean 1.2-1.3 levels, p99 4-5, max 7-8
+    # bound for bf16 GPU-vs-CPU differences after resampling
     assert d.mean() <= 2.5 and np.percentile(d, 99) <= 12, f"{name}: mean {d.mean():.2f}, p99 {np.percentile(d, 99)}"
 
 

@@ -1,4 +1,4 @@
-"""-m gpu: the product path (bagel_b200 host code -> C ABI -> sm_100a kernels) against the committed reference
+"""-m gpu: the product path (bagel_b200 host code -> C ABI -> sm_90a kernels) against the committed reference
 outputs (tests/golden) and the oracle.
 
 Tolerance model. The reference is a bf16 pipeline (autocast): its own outputs carry bf16 rounding noise, and any

@@ -44,15 +44,15 @@ def _ev_ms(fn, iters: int, warm: int = 3) -> float:
 def attn_block(peaks: Dict, dev, iters: int = 10) -> Dict:
     """SURVEY.md §8d cfg 5: bf16, d=128, Hq=32 (MHA 32:32 as written, and the model's 28:4 GQA); L in {1k,4k,16k} x
     {uniform non-causal, causal, ragged (lengths randint(L/2, L), seed 5)}; plus the denoise shapes q=4098 vs
-    kv=4098+{66, 9066}. 16384 packed query tokens per call -> q/k/v/out are 134 MB each (> the 126 MB L2, so successive
+    kv=4098+{66, 9066}. 16384 packed query tokens per call -> q/k/v/out are 134 MB each (> the 50 MB L2, so successive
     iterations do not find their inputs cached). FLOPs = 4*sum(Lq*Lk)*Hq*d (/2 causal)."""
     from bagel_b200 import ops
     try:
         from flash_attn import flash_attn_varlen_func
     except Exception:
         flash_attn_varlen_func = None
-    burst = float(peaks.get("bf16_tflops", 1636.0))
-    hbm = float(peaks.get("hbm_gbs", 6582.5))
+    burst = float(peaks.get("bf16_tflops", 989.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
     g = torch.Generator(device=dev).manual_seed(4)
     rows: List[Dict] = []
 
@@ -93,15 +93,16 @@ def attn_block(peaks: Dict, dev, iters: int = 10) -> Dict:
     one("denoise q=4098 kv=4164 B=4", 28, 4, [4098] * 4, [4164] * 4, False)
     one("denoise q=4098 kv=13164 B=4 (edit ctx)", 28, 4, [4098] * 4, [13164] * 4, False)
     best = max(rows, key=lambda r: r["tflops"])
-    return {"peak_tflops_burst": burst, "peak_source": "MEASURED_PEAKS.json bf16_tflops (kernel timed alone)",
-            "l2": "inputs > 126 MB L2 (16384 packed query tokens per call)", "iters": iters, "shapes": rows,
+    return {"peak_tflops_burst": burst, "peak_source": "bench.py measured_peaks() bf16_tflops",
+            "l2": "inputs > 50 MB L2 (16384 packed query tokens per call)", "iters": iters, "shapes": rows,
             "best_tflops": best["tflops"], "best_shape": best["shape"]}
 
 
 # ----------------------------------------------------------------------------------------------------------------
 # configs[2]: understanding prefill, Bagel.chat call order, batch 32; and the decode step on top of that context
 # ----------------------------------------------------------------------------------------------------------------
-def und_prefill_and_decode_block(model, dev, batch: int = 32, text_tokens: int = 512, decode: bool = True) -> Dict:
+def und_prefill_and_decode_block(model, dev, batch: int = 32, text_tokens: int = 512, decode: bool = True,
+                                 hbm_gbs: float = 3350.0) -> Dict:
     """32 synthetic 378x378 PIL images -> VLM transform ImageTransform(980, 378, 14, max_pixels=2_007_040)
     (data/configs/example.yaml:32-36: 378^2 stays 378^2 = 729 patches) -> prepare_vit_images -> forward_cache_update_vit
     -> prepare_prompts (512 random ids + bos/eos) -> forward_cache_update_text: the order of Bagel.chat
@@ -172,8 +173,8 @@ def und_prefill_and_decode_block(model, dev, batch: int = 32, text_tokens: int =
                                      "steady state = (min t[144 steps] - min t[16 steps]) / 128 over two rounds after a warm-up call",
                          "calls_s": [[s_, round(t, 4)] for s_, t in calls],
                          "ms_per_step": ms, "tokens_per_s": batch / ms * 1e3,
-                         "hbm_bytes_per_step": wbytes + kvbytes, "hbm_roofline_ms": (wbytes + kvbytes) / 6582.5e6,
-                         "frac_of_hbm_roofline": (wbytes + kvbytes) / 6582.5e6 / ms}
+                         "hbm_bytes_per_step": wbytes + kvbytes, "hbm_roofline_ms": (wbytes + kvbytes) / (hbm_gbs * 1e6),
+                         "frac_of_hbm_roofline": (wbytes + kvbytes) / (hbm_gbs * 1e6) / ms}
     return out
 
 
@@ -271,5 +272,5 @@ def library_baseline_and_parity(model, gen_input, cfg_text_input, ctx_main, gen_
            "ratio_to_noise_floor": got["rel_l2"] / max(floor["rel_l2"], 1e-30),
            "velocity_rel_l2": {"product_vs_reference": dv((x0 - x1) / dt0, v_fa2.float()),
                                "noise_floor": dv(v_sdpa.float(), v_fa2.float())},
-           "full_run_drift": "profiles/r02_drift_7b.txt (28 layers x 49 steps incl. fp32 truth), tests/test_gpu_drift_7b.py"}
+           "full_run_drift": "tests/test_gpu_drift_7b.py (28 layers x 49 steps incl. fp32 truth)"}
     return {"gpu_library_baseline": lib, "parity": par}

@@ -17,5 +17,5 @@ obj = out_dir / f"{stem}_{name}.o"
 subprocess.check_call([bb._nvcc(), *bb.NVCC_FLAGS, *flags, "-c", str(bb.CSRC / f"{stem}.cu"), "-o", str(obj)])
 objs = [str(o) for o in sorted((bb.PKG_DIR / "build").glob("*.o")) if o.name != f"{stem}.o"] + [str(obj)]
 lib = out_dir / f"libbagel_b200_{name}.so"
-subprocess.check_call([bb._nvcc(), "-shared", "-o", str(lib), *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcuda"])
+subprocess.check_call([bb._nvcc(), "-shared", "-o", str(lib), *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcuda"])
 print("built", lib)

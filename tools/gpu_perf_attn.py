@@ -1,4 +1,4 @@
-"""Attention microbench (BASELINE configs[4]): packed varlen, d=128, bf16; ours vs flash_attn 2.8 (FA2 SASS on sm_100)."""
+"""Attention microbench (BASELINE configs[4]): packed varlen, d=128, bf16; ours vs flash_attn 2.8 (FA2 on the same GPU)."""
 import sys, torch
 sys.path.insert(0, ".")
 import os
