@@ -15,14 +15,15 @@ What is different underneath (GPU-first, not a port):
 """
 from __future__ import annotations
 
-from typing import Any, Dict, List, Optional, Sequence, Tuple
+import warnings
+from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
 from . import ops
 from .config import BagelConfig
 from .modeling_utils import MLPconnector, PositionEmbedding, TimestepEmbedder
-from .qwen2_navit import NaiveCache, Qwen2ForCausalLM
+from .qwen2_navit import ForwardPlan, NaiveCache, Qwen2ForCausalLM, _ranges
 
 BF16 = torch.bfloat16
 
@@ -30,16 +31,6 @@ BF16 = torch.bfloat16
 # --------------------------------------------------------------------------------------------------
 # index helpers (host, int64)
 # --------------------------------------------------------------------------------------------------
-def _ranges(starts: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
-    """concat_i arange(starts[i], starts[i] + lens[i])"""
-    lens = lens.to(torch.int64)
-    total = int(lens.sum())
-    if total == 0:
-        return torch.zeros(0, dtype=torch.int64)
-    excl = torch.cumsum(lens, 0) - lens
-    return torch.repeat_interleave(starts.to(torch.int64) - excl, lens) + torch.arange(total, dtype=torch.int64)
-
-
 def get_flattened_position_ids_extrapolate(img_h, img_w, patch_size, max_num_patches_per_side):
     """row * max_side + col for every patch (reference data/data_utils.py:53-58)."""
     nh, nw = img_h // patch_size, img_w // patch_size
@@ -62,6 +53,36 @@ def patchify(image: torch.Tensor, patch_size: int) -> torch.Tensor:
     p = patch_size
     assert h % p == 0 and w % p == 0
     return image.reshape(c, h // p, p, w // p, p).permute(1, 3, 2, 4, 0).reshape(-1, p * p * c)
+
+
+def _cfg_branches(main, text, img, cfg_text_scale: float, cfg_img_scale: float) -> List[Dict[str, Any]]:
+    """The LM calls of one CFG velocity evaluation: the conditional branch, the text-CFG branch when
+    cfg_text_scale > 1 and, only inside it, the image-CFG branch (the reference consumes the image branch only
+    inside the text-CFG block, :873). Each argument is (packed_position_ids, packed_query_indexes, past_key_values,
+    key_values_lens, packed_key_value_indexes)."""
+    names = ("packed_position_ids", "packed_query_indexes", "past_key_values", "key_values_lens",
+             "packed_key_value_indexes")
+    branches = [main]
+    if cfg_text_scale > 1.0:
+        branches.append(text)
+        if cfg_img_scale > 1.0:
+            branches.append(img)
+    return [dict(zip(names, b)) for b in branches]
+
+
+def _capture_graph(launch: Callable[[], None], what: str) -> Optional[torch.cuda.CUDAGraph]:
+    """Capture launch() as a CUDA graph and replay it once (capture does not execute the work). Capture is an
+    optimisation and the eager launch sequence is the same work: on failure, warn, synchronise and return None."""
+    try:
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            launch()
+        graph.replay()
+        return graph
+    except Exception as e:
+        warnings.warn(f"bagel_b200: CUDA graph capture of {what} failed, continuing eagerly: {e}")
+        torch.cuda.synchronize()
+        return None
 
 
 class _Affine:
@@ -427,19 +448,14 @@ class Bagel:
             vae.append(torch.as_tensor(packed_vae_token_indexes).to("cpu", torch.int64) + b * n)
             txt.append(torch.as_tensor(packed_text_indexes).to("cpu", torch.int64) + b * n)
             row_off += total_b
-        plan = lm.make_plan(query_lens=torch.cat(ql), position_ids=torch.cat(pos),
-                            packed_query_indexes=torch.cat(qidx), key_values_lens=torch.cat(kvl),
-                            packed_key_value_indexes=torch.cat(kvidx), is_causal=False,
-                            mode="gen" if self.use_moe else "und",
-                            packed_vae_token_indexes=torch.cat(vae), packed_text_indexes=torch.cat(txt))
+        plan = ForwardPlan(lm, query_lens=torch.cat(ql), position_ids=torch.cat(pos),
+                           packed_query_indexes=torch.cat(qidx), key_values_lens=torch.cat(kvl),
+                           packed_key_value_indexes=torch.cat(kvidx), is_causal=False,
+                           mode="gen" if self.use_moe else "und",
+                           packed_vae_token_indexes=torch.cat(vae), packed_text_indexes=torch.cat(txt))
         kbuf, vbuf = lm.alloc_kv(plan)
-        cfg = lm.config
-        w = cfg.num_key_value_heads * cfg.head_dim
         for cache, rows in ctx_pairs:
-            m = rows.numel()
-            for li in range(cfg.num_hidden_layers):
-                ops.copy_rows(cache.key_cache[li].reshape(m, w), kbuf[li], dst_rows=rows, M=m)
-                ops.copy_rows(cache.value_cache[li].reshape(m, w), vbuf[li], dst_rows=rows, M=m)
+            lm.place_context(cache, rows, kbuf, vbuf)
         return plan, kbuf, vbuf
 
     def _velocity(self, st: Dict[str, Any], key: str, t_row: torch.Tensor, x_src: torch.Tensor, head: bool = True) -> int:
@@ -529,20 +545,12 @@ class Bagel:
         ts = ts[:-1]
         cfg_on = [bool(t > cfg_interval[0] and t <= cfg_interval[1]) for t in ts]
 
-        main = dict(packed_position_ids=packed_position_ids, packed_query_indexes=packed_indexes,
-                    past_key_values=past_key_values, key_values_lens=key_values_lens,
-                    packed_key_value_indexes=packed_key_value_indexes)
-        branches = [main]
-        if cfg_text_scale > 1.0:
-            branches.append(dict(packed_position_ids=cfg_text_packed_position_ids,
-                                 packed_query_indexes=cfg_text_packed_query_indexes,
-                                 past_key_values=cfg_text_past_key_values, key_values_lens=cfg_text_key_values_lens,
-                                 packed_key_value_indexes=cfg_text_packed_key_value_indexes))
-            if cfg_img_scale > 1.0:  # the reference consumes the image branch only inside the text-CFG block (:873)
-                branches.append(dict(packed_position_ids=cfg_img_packed_position_ids,
-                                     packed_query_indexes=cfg_img_packed_query_indexes,
-                                     past_key_values=cfg_img_past_key_values, key_values_lens=cfg_img_key_values_lens,
-                                     packed_key_value_indexes=cfg_img_packed_key_value_indexes))
+        branches = _cfg_branches(
+            (packed_position_ids, packed_indexes, past_key_values, key_values_lens, packed_key_value_indexes),
+            (cfg_text_packed_position_ids, cfg_text_packed_query_indexes, cfg_text_past_key_values,
+             cfg_text_key_values_lens, cfg_text_packed_key_value_indexes),
+            (cfg_img_packed_position_ids, cfg_img_packed_query_indexes, cfg_img_past_key_values,
+             cfg_img_key_values_lens, cfg_img_packed_key_value_indexes), cfg_text_scale, cfg_img_scale)
         nbmax = len(branches)
         # every LM workspace at its final size BEFORE the first launch / graph capture: the 'full' (all-branch) steps
         # need nbmax*n rows, the 'main' steps n — growing a buffer in between would free memory a captured graph replays into
@@ -582,119 +590,70 @@ class Bagel:
         GPU-first execution (the reference re-allocates and re-scatters the whole KV cache per layer per token and
         rebuilds index tensors with host loops): the KV cache is copied ONCE into per-sample slabs with room for
         `max_length` new tokens; sequence lengths, RoPE positions, write slots and the token history live on the
-        device; a step is embedding gather -> 28 layers (fused QKV epilogue appends K/V in place, attention reads
-        `seqused_k`) -> final norm -> lm_head -> argmax, captured once as a CUDA graph and replayed per token.
-        The only host<->device traffic per step is the 8-byte EOS check the reference also performs."""
+        device. A step is embedding gather -> `run_layers` on a decode `ForwardPlan` (the QKV projection appends K/V
+        in place, attention reads `seqused_k`) -> final norm -> lm_head -> argmax, captured once as a CUDA graph and
+        replayed per token. The only host<->device traffic per step is the 8-byte EOS check the reference also
+        performs."""
         dev = self.device
         lm = self.language_model.model
         if self.dtype_mode == "B":
             raise NotImplementedError("generate_text: the device-resident decode loop is implemented for dtype_mode='A'")
         cfg = lm.config
-        L, H, Hq, Hk, D = cfg.num_hidden_layers, cfg.hidden_size, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        w = Hk * D
+        L, w = cfg.num_hidden_layers, cfg.num_key_value_heads * cfg.head_dim
         kv = torch.as_tensor(key_values_lens).to("cpu", torch.int64)
         B = int(kv.numel())
         if max_length <= 0:
             return torch.zeros((0, B), dtype=torch.int64, device=dev)
-        cap = kv + max_length
-        begin = torch.cumsum(cap, 0) - cap
-        total = int(cap.sum())
-        max_kv = int(cap.max())   # host upper bound of any sample's key count (sizes the key split of decode attention)
-        has_ctx = past_key_values is not None and past_key_values.key_cache[0] is not None and int(kv.sum()) > 0
+        plan = ForwardPlan.decode(lm, kv, max_length)
         # zero-filled, not torch.empty: attention multiplies the masked probabilities (exactly 0) with whatever sits in the
         # spare rows of a slab — 0 x NaN/Inf garbage would poison the output (the attention kernel fetches whole 128-key
         # blocks by TMA; only the single-query d=128 kernel clamps its loads to the rows in use)
-        kbuf = torch.zeros((L, total, w), dtype=BF16, device=dev)
-        vbuf = torch.zeros((L, total, w), dtype=BF16, device=dev)
-        if has_ctx:
-            n_ctx = int(kv.sum())
-            dst = _ranges(begin, kv).to(dev, torch.int32)
-            for li in range(L):
-                ops.copy_rows(past_key_values.key_cache[li].reshape(n_ctx, w), kbuf[li], dst_rows=dst, M=n_ctx)
-                ops.copy_rows(past_key_values.value_cache[li].reshape(n_ctx, w), vbuf[li], dst_rows=dst, M=n_ctx)
-        k_begin = torch.cat([begin, torch.tensor([total])]).to(dev, torch.int32)
-        cu_q = torch.arange(B + 1, dtype=torch.int32, device=dev)
+        kbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
+        vbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
+        if past_key_values is not None and past_key_values.key_cache[0] is not None and plan.n_ctx:
+            lm.place_context(past_key_values, plan.ctx_rows, kbuf, vbuf)
         seq_len = kv.to(dev, torch.int32)
         pos = torch.as_tensor(packed_query_position_ids).to(dev, torch.int64).clone()
         tokens = torch.as_tensor(packed_start_tokens).to(dev, torch.int64).clone()
         tokens32 = tokens.to(torch.int32)
         history = torch.zeros((max_length, B), dtype=torch.int64, device=dev)
         step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
-        kv_rows = torch.zeros(B, dtype=torch.int32, device=dev)
-        seqused = torch.zeros(B, dtype=torch.int32, device=dev)
-        x = torch.empty((B, H), dtype=BF16, device=dev)
+        x = lm._buf("xa", B, cfg.hidden_size)      # run_layers' input workspace: the gather needs no extra copy
         logits = torch.empty((B, cfg.vocab_size), dtype=BF16, device=dev)
-        eps = cfg.rms_norm_eps
-        bufs = dict(xb=torch.empty_like(x), h=torch.empty_like(x),
-                    qkv=torch.empty((B, (Hq + 2 * Hk) * D), dtype=BF16, device=dev),
-                    q=torch.empty((B, Hq * D), dtype=BF16, device=dev), att=torch.empty((B, Hq * D), dtype=BF16, device=dev),
-                    act=torch.empty((B, cfg.intermediate_size), dtype=BF16, device=dev), out=torch.empty_like(x))
         head = self.language_model.lm_head
 
         def body():
             """One decode step; every input/output is a fixed device buffer (graph-replayable)."""
             ops.copy_rows(lm.embed_tokens.weight, x, src_rows=tokens32, M=B)
-            cos, sin = bufs.get("cos"), bufs.get("sin")
-            ops.rope_table_into(pos, lm.inv_freq, cos, sin, True)
-            ops.decode_prepare(k_begin, seq_len, kv_rows, seqused)
-            xa, xb, h = x, bufs["xb"], bufs["h"]
-            for li, layer in enumerate(lm.layers):
-                e = layer.und
-                ops.rmsnorm(xa, e.ln_in, None, None, eps, out=h)
-                if lm.fused_qkv and D == 128 and B > 64:   # B <= 64: weight-streaming skinny GEMM + norm/RoPE kernel
-                    ops.gemm_qkv_norm_rope(h, e.wqkv, e.bqkv, e.q_norm, e.k_norm, None, None, None, cos, sin, bufs["q"],
-                                           kbuf[li], vbuf[li], kv_rows, Hq, Hk, eps, False)
-                else:
-                    ops.gemm(h, e.wqkv, bias=e.bqkv, out=bufs["qkv"])
-                    ops.qk_norm_rope(bufs["qkv"], e.q_norm, e.k_norm, None, None, None, cos, sin, bufs["q"], kbuf[li],
-                                     vbuf[li], kv_rows, Hq, Hk, D, eps, False)
-                ops.attn_varlen(bufs["q"].view(B, Hq, D), kbuf[li].view(-1, Hk, D), vbuf[li].view(-1, Hk, D), cu_q, k_begin,
-                                1, max_kv, True, out=bufs["att"].view(B, Hq, D), seqused_k=seqused)
-                ops.gemm(bufs["att"], e.wo, resid=xa, epilogue=ops.EPI_RESID, out=xb)
-                ops.rmsnorm(xb, e.ln_post, None, None, eps, out=h)
-                ops.gemm(h, e.wgu, epilogue=ops.EPI_SWIGLU, out=bufs["act"])
-                ops.gemm(bufs["act"], e.wd, resid=xb, epilogue=ops.EPI_RESID, out=xa)
-            ops.rmsnorm(xa, lm.norm, None, None, eps, out=bufs["out"])
-            ops.gemm(bufs["out"], head.weight, bias=head.bias, out=logits)
+            ops.rope_table_into(pos, lm.inv_freq, plan.cos, plan.sin, True)
+            ops.decode_prepare(plan.cu_k, seq_len, plan.q_rows, plan.seqused_k)
+            out = lm.run_layers(x, plan, kbuf, vbuf)     # decoder layers + final norm
+            ops.gemm(out, head.weight, bias=head.bias, out=logits)
 
-        def tail_greedy():
+        def greedy_step():
+            body()
             ops.decode_advance(seq_len, pos, tokens, history, step_dev)   # history[step] = current tokens; lens += 1
             ops.argmax_rows(logits, tokens, tokens32)
 
-        bufs["cos"] = torch.empty((B, D // 2), dtype=torch.float32, device=dev)
-        bufs["sin"] = torch.empty((B, D // 2), dtype=torch.float32, device=dev)
         graph = None
-        use_graph = bool(getattr(self, "use_cuda_graph", True)) and not do_sample
         steps = 0
         for step in range(max_length):
             if graph is not None:
                 graph.replay()
+            elif do_sample:
+                body()
+                ops.decode_advance(seq_len, pos, tokens, history, step_dev)
+                probs = torch.softmax(logits.float() / temperature, dim=-1)
+                nxt = torch.multinomial(probs, num_samples=1).squeeze(1)
+                tokens.copy_(nxt)
+                tokens32.copy_(nxt.to(torch.int32))
+            elif step == 1 and self.use_cuda_graph:
+                # step 0 ran eagerly and sized every LM workspace the step uses, so the capture allocates none
+                graph = _capture_graph(greedy_step, "the decode step")
+                if graph is None:
+                    greedy_step()
             else:
-                if use_graph and step == 1:
-                    try:
-                        g = torch.cuda.CUDAGraph()
-                        with torch.cuda.graph(g):
-                            body()
-                            tail_greedy()
-                        graph = g
-                        graph.replay()
-                    except Exception as e:
-                        use_graph = False
-                        import warnings
-                        warnings.warn(f"bagel_b200: CUDA graph capture of the decode step failed, continuing eagerly: {e}")
-                        torch.cuda.synchronize()
-                        body()
-                        tail_greedy()
-                else:
-                    body()
-                    if do_sample:
-                        ops.decode_advance(seq_len, pos, tokens, history, step_dev)
-                        probs = torch.softmax(logits.float() / temperature, dim=-1)
-                        nxt = torch.multinomial(probs, num_samples=1).squeeze(1)
-                        tokens.copy_(nxt)
-                        tokens32.copy_(nxt.to(torch.int32))
-                    else:
-                        tail_greedy()
+                greedy_step()
             steps += 1
             if end_token_id is not None and int(tokens[0]) == end_token_id:
                 break
@@ -870,23 +829,14 @@ class Bagel:
             raise NotImplementedError("TaylorSeer caches are not accepted by _forward_flow; use "
                                       "generate_image(..., enable_taylorseer=True)")
         dev = self.device
-        lm = self.language_model.model
         t = torch.as_tensor(timestep).to("cpu", torch.float32).reshape(-1)
         assert t.unique().numel() == 1
-        main = dict(packed_position_ids=packed_position_ids, packed_query_indexes=packed_indexes,
-                    past_key_values=past_key_values, key_values_lens=key_values_lens,
-                    packed_key_value_indexes=packed_key_value_indexes)
-        branches = [main]
-        if cfg_text_scale > 1.0:
-            branches.append(dict(packed_position_ids=cfg_text_packed_position_ids,
-                                 packed_query_indexes=cfg_text_packed_query_indexes,
-                                 past_key_values=cfg_text_past_key_values, key_values_lens=cfg_text_key_values_lens,
-                                 packed_key_value_indexes=cfg_text_packed_key_value_indexes))
-            if cfg_img_scale > 1.0:
-                branches.append(dict(packed_position_ids=cfg_img_packed_position_ids,
-                                     packed_query_indexes=cfg_img_packed_query_indexes,
-                                     past_key_values=cfg_img_past_key_values, key_values_lens=cfg_img_key_values_lens,
-                                     packed_key_value_indexes=cfg_img_packed_key_value_indexes))
+        branches = _cfg_branches(
+            (packed_position_ids, packed_indexes, past_key_values, key_values_lens, packed_key_value_indexes),
+            (cfg_text_packed_position_ids, cfg_text_packed_query_indexes, cfg_text_past_key_values,
+             cfg_text_key_values_lens, cfg_text_packed_key_value_indexes),
+            (cfg_img_packed_position_ids, cfg_img_packed_query_indexes, cfg_img_past_key_values,
+             cfg_img_key_values_lens, cfg_img_packed_key_value_indexes), cfg_text_scale, cfg_img_scale)
         nb = len(branches)
         st = self._flow_state(x_t, packed_seqlens, packed_vae_token_indexes, packed_text_indexes,
                               packed_vae_position_ids, packed_text_ids, nb)
@@ -991,19 +941,13 @@ class FlowRunner:
             # the graph holds pointers into freed buffers -> drop it and capture again on the current ones
             del self._graphs[key]
         if self.use_cuda_graph and self._eager_done.get(key, 0) >= 1:
-            try:  # everything is warm (workspaces allocated, kernel attributes set): capture this step
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    self._body(key)
+            # everything is warm (workspaces allocated, kernel attributes set): capture this step
+            graph = _capture_graph(lambda: self._body(key), "the denoising step")
+            if graph is not None:
                 self._graphs[key] = graph
                 self._graph_gen[key] = lm._ws_gen
-                graph.replay()          # capture does not execute the work
                 return
-            except Exception as e:  # capture is an optimisation; the eager launch sequence is the same work
-                self.use_cuda_graph = False
-                import warnings
-                warnings.warn(f"bagel_b200: CUDA graph capture failed, continuing eagerly: {e}")
-                torch.cuda.synchronize()
+            self.use_cuda_graph = False
         self._body(key)
         self._eager_done[key] = self._eager_done.get(key, 0) + 1
 

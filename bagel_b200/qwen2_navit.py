@@ -30,6 +30,16 @@ from .config import Qwen2Config
 BF16 = torch.bfloat16
 
 
+def _ranges(starts: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
+    """concat_i arange(starts[i], starts[i] + lens[i])"""
+    lens = lens.to(torch.int64)
+    total = int(lens.sum())
+    if total == 0:
+        return torch.zeros(0, dtype=torch.int64)
+    excl = torch.cumsum(lens, 0) - lens
+    return torch.repeat_interleave(starts.to(torch.int64) - excl, lens) + torch.arange(total, dtype=torch.int64)
+
+
 class NaiveCache:
     """Per-layer packed KV tensors [sum_kv, Hk, D] (or None) — reference qwen2_navit.py:207-221.
     Deep-copyable (inferencer.py:230-253 relies on copy.deepcopy of whole contexts)."""
@@ -92,14 +102,19 @@ class _Layer:
 
 class ForwardPlan:
     """Everything about one packed LM call that does not depend on the hidden states: int32 index maps on the
-    device, cu_seqlens, RoPE tables. Built once per call (or once per denoising run) so the layer loop is pure
-    kernel launches with no host<->device synchronisation (the reference syncs >= 2x per layer, :585-586)."""
+    device, cu_seqlens, RoPE tables, which QKV path runs. Built once per call (or once per denoising run, or once
+    per decode) so the layer loop is pure kernel launches with no host<->device synchronisation (the reference
+    syncs >= 2x per layer, :585-586). The constructor plans a packed prefill / denoising call; `decode()` plans
+    the one-token-per-sample step of text generation."""
 
     def __init__(self, lm: "Qwen2Model", query_lens, position_ids, packed_query_indexes, key_values_lens,
                  packed_key_value_indexes, is_causal: bool, mode: str, packed_vae_token_indexes=None,
                  packed_text_indexes=None, train_numerics: bool = False):
         dev = lm.device
         cfg = lm.config
+        # head_dim 128: q/k-norm + RoPE + KV placement fused into the QKV GEMM epilogue
+        self.fuse_qkv = cfg.head_dim == 128
+        self.seqused_k = None
         ql = torch.as_tensor(query_lens).to("cpu", torch.int64).reshape(-1)
         self.batch = int(ql.numel())
         self.n = int(ql.sum())
@@ -129,6 +144,7 @@ class ForwardPlan:
         self.q_rows = torch.as_tensor(packed_query_indexes).to(dev, torch.int32).contiguous()
         if self.n_ctx:
             self.ctx_rows = torch.as_tensor(packed_key_value_indexes).to(dev, torch.int32).contiguous()
+            assert self.ctx_rows.numel() == self.n_ctx, "one packed key/value index per context row"
         else:
             self.ctx_rows = None
         self.expert = None
@@ -144,6 +160,33 @@ class ForwardPlan:
         assert pos.numel() == self.n, "one position id per packed query token"
         # cos/sin take the dtype of the hidden stream (bf16 in mode A, fp32 in mode B): modeling_qwen2.py:150
         self.cos, self.sin = ops.rope_table(pos, lm.inv_freq, round_bf16=(lm.dtype_mode == "A"))
+
+    @classmethod
+    def decode(cls, lm: "Qwen2Model", key_values_lens, max_length: int) -> "ForwardPlan":
+        """One new token per sample against per-sample K/V slabs: sample i owns rows [cu_k[i], cu_k[i+1]), its
+        key_values_lens[i] context rows (ctx_rows) followed by room for `max_length` new ones. The per-step state is
+        device-resident so that a step is replayable as a CUDA graph: ops.decode_prepare fills q_rows (the slab row each
+        new K/V is written to) and seqused_k (keys in use), ops.rope_table_into fills cos/sin."""
+        dev, D = lm.device, lm.config.head_dim
+        kv = torch.as_tensor(key_values_lens).to("cpu", torch.int64).reshape(-1)
+        cap = kv + max_length
+        begin = torch.cumsum(cap, 0) - cap
+        p = cls.__new__(cls)
+        p.batch = p.n = B = int(kv.numel())
+        p.n_ctx, p.total_kv = int(kv.sum()), int(cap.sum())
+        p.max_q = 1
+        p.max_k = int(cap.max())   # host upper bound of any sample's key count (sizes the key split of decode attention)
+        p.cu_q = torch.arange(B + 1, dtype=torch.int32, device=dev)
+        p.cu_k = torch.cat([begin, torch.tensor([p.total_kv])]).to(dev, torch.int32)
+        p.ctx_rows = _ranges(begin, kv).to(dev, torch.int32)
+        p.q_rows = torch.zeros(B, dtype=torch.int32, device=dev)
+        p.seqused_k = torch.zeros(B, dtype=torch.int32, device=dev)
+        p.cos = torch.empty((B, D // 2), dtype=torch.float32, device=dev)
+        p.sin = torch.empty((B, D // 2), dtype=torch.float32, device=dev)
+        p.is_causal, p.mode, p.fp32_flow = True, "und", 0
+        p.expert = p.text_rows = None
+        p.fuse_qkv = D == 128 and B > 64   # B <= 64: weight-streaming skinny GEMM + norm/RoPE kernel
+        return p
 
 
 class Qwen2Model:
@@ -163,7 +206,6 @@ class Qwen2Model:
         self.layer_kind = kinds[config.layer_module]
         self.use_moe = "Mo" in config.layer_module      # same test as the reference (:948): MoE and MoT
         self.enable_taylorseer = False
-        self.fused_qkv = True   # head_dim 128: q/k-norm + RoPE + KV placement fused into the QKV GEMM epilogue
         self.layers: List[_Layer] = [_Layer() for _ in range(config.num_hidden_layers)]
         self.embed_tokens: Optional[_Embedding] = None
         self.norm = None
@@ -198,9 +240,6 @@ class Qwen2Model:
             for name, cols in (("h_text", H), ("att_text", Hq * D), ("act_text", I)):
                 self._buf(name, text_rows, cols)
 
-    def make_plan(self, **kw) -> ForwardPlan:
-        return ForwardPlan(self, **kw)
-
     def alloc_kv(self, plan: ForwardPlan):
         """Merged K/V buffers [total_kv, Hk*D] for every layer (the reference re-allocates these per layer per
         call, qwen2_navit.py:563-569)."""
@@ -211,17 +250,16 @@ class Qwen2Model:
         v = torch.empty((L, plan.total_kv, w), dtype=BF16, device=self.device)
         return k, v
 
-    def place_context(self, plan: ForwardPlan, cache: Optional[NaiveCache], kbuf, vbuf):
-        """Copy the cached K/V rows to their slots in the merged buffers (reference :565-569)."""
-        if not plan.n_ctx:
-            return
+    def place_context(self, cache: NaiveCache, rows: torch.Tensor, kbuf, vbuf):
+        """Copy every layer's cached K/V rows to `rows` (int32, on the device) of the merged buffers (reference
+        :565-569)."""
         cfg = self.config
-        w = cfg.num_key_value_heads * cfg.head_dim
+        m, w = rows.numel(), cfg.num_key_value_heads * cfg.head_dim
         for li in range(cfg.num_hidden_layers):
             pk, pv = cache.key_cache[li], cache.value_cache[li]
-            assert pk is not None and pk.shape[0] == plan.n_ctx, "cache rows must match key_values_lens"
-            ops.copy_rows(pk.reshape(plan.n_ctx, w), kbuf[li], dst_rows=plan.ctx_rows, M=plan.n_ctx)
-            ops.copy_rows(pv.reshape(plan.n_ctx, w), vbuf[li], dst_rows=plan.ctx_rows, M=plan.n_ctx)
+            assert pk is not None and pk.shape[0] == m, "cache rows must match key_values_lens"
+            ops.copy_rows(pk.reshape(m, w), kbuf[li], dst_rows=rows, M=m)
+            ops.copy_rows(pv.reshape(m, w), vbuf[li], dst_rows=rows, M=m)
 
     # ----------------------------------------------------------------------------------------------
     def run_layers(self, x: torch.Tensor, plan: ForwardPlan, kbuf: torch.Tensor, vbuf: torch.Tensor,
@@ -264,7 +302,7 @@ class Qwen2Model:
             amain = layer.gen if a_routed else layer.und     # norm / attention weights every row runs through
             # ---- attention block ----
             rmsnorm(xa, und.ln_in, amain.ln_in if a_routed else None, a_expert, eps, out=h)
-            if self.fused_qkv and D == 128:
+            if plan.fuse_qkv:
                 # QKV GEMM with q/k-norm + RoPE + KV placement in its epilogue (no [n, 4608] round trip)
                 ops.gemm_qkv_norm_rope(h, amain.wqkv, amain.bqkv, und.q_norm, und.k_norm,
                                        amain.q_norm if a_routed else None, amain.k_norm if a_routed else None, a_expert,
@@ -283,7 +321,7 @@ class Qwen2Model:
                                  amain.k_norm if a_routed else None, a_expert, plan.cos, plan.sin, q, kbuf[li], vbuf[li],
                                  plan.q_rows, Hq, Hk, D, eps, plan.fp32_flow)
             ops.attn_varlen(q.view(n, Hq, D), kbuf[li].view(-1, Hk, D), vbuf[li].view(-1, Hk, D), plan.cu_q, plan.cu_k,
-                            plan.max_q, plan.max_k, plan.is_causal, out=att.view(n, Hq, D))
+                            plan.max_q, plan.max_k, plan.is_causal, out=att.view(n, Hq, D), seqused_k=plan.seqused_k)
             ops.gemm(att, amain.wo, resid=xa, epilogue=EPI_R, out=xb)
             if nta:
                 ops.copy_rows(att, at, src_rows=plan.text_rows)
@@ -333,7 +371,8 @@ class Qwen2Model:
                            is_causal, mode, packed_vae_token_indexes, packed_text_indexes, train_numerics)
         x = packed_query_sequence.to(self.device, self.stream_dtype)
         kbuf, vbuf = self.alloc_kv(plan)
-        self.place_context(plan, past_key_values, kbuf, vbuf)
+        if plan.n_ctx:
+            self.place_context(past_key_values, plan.ctx_rows, kbuf, vbuf)
         out = self.run_layers(x, plan, kbuf, vbuf).clone()
         if update_past_key_values:
             cfg = self.config
