@@ -39,17 +39,6 @@ __device__ __forceinline__ float ex2f(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ float ld_dsmem_f32(const float* local, uint32_t rank) {
-  uint32_t remote;
-  float v;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(local)), "r"(rank));
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
-  return v;
-}
 
 // m16n8k16 bf16 x bf16 -> fp32 (legacy warp-level tensor-core path; the 7-8 query heads of a GQA group are the M rows)
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
@@ -257,9 +246,9 @@ __global__ void __launch_bounds__(kThreads, 2) attn_decode_kernel(const DecodePa
 #pragma unroll
       for (int r = 0; r < kMaxSplit; ++r) {
         const bool on = r < p.split;
-        mr[r] = !on ? -INFINITY : (p.split > 1 ? ld_dsmem_f32(&part_m[h], r) : part_m[h]);
-        lr[r] = !on ? 0.f : (p.split > 1 ? ld_dsmem_f32(&part_l[h], r) : part_l[h]);
-        ar[r] = !on ? 0.f : (p.split > 1 ? ld_dsmem_f32(&part_acc[h][t], r) : part_acc[h][t]);
+        mr[r] = !on ? -INFINITY : (p.split > 1 ? ld_dsmem_f32(smem_u32(&part_m[h]), r) : part_m[h]);
+        lr[r] = !on ? 0.f : (p.split > 1 ? ld_dsmem_f32(smem_u32(&part_l[h]), r) : part_l[h]);
+        ar[r] = !on ? 0.f : (p.split > 1 ? ld_dsmem_f32(smem_u32(&part_acc[h][t]), r) : part_acc[h][t]);
       }
       float M = -INFINITY;
 #pragma unroll

@@ -73,6 +73,37 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// thread-block clusters: rank, cluster-wide barrier, distributed shared memory
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// Every thread of every CTA of the cluster (aligned: each warp converged).
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// Address of the same shared-memory offset in the CTA of rank `rank` of this cluster.
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local_addr), "r"(rank));
+  return remote;
+}
+__device__ __forceinline__ float ld_dsmem_f32(uint32_t local_addr, uint32_t rank) {
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(mapa_shared(local_addr, rank)) : "memory");
+  return v;
+}
+// Arrive on the mbarrier at the same offset in the CTA of rank `rank` (default semantics: release at CTA scope). Meant for
+// handing back a slot whose readers were async-proxy operations that have already completed (wgmma after
+// wgmma.wait_group): a .release.cluster arrive would put a MEMBAR.GPU in front of every arrive.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa_shared(smem_u32(bar), rank)) : "memory");
+}
+
 // Exactly one lane of a CONVERGED warp (elect.sync): guards single-thread TMA issue; with it ptxas knows that one thread
 // runs the region, behind `lane == 0` it has to assume divergence.
 __device__ __forceinline__ bool elect_one_lane() {
@@ -116,6 +147,17 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       " [%0], [%1, {%3, %4}], [%2], %5;"
       ::"r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
+      : "memory");
+}
+// The box lands at the same shared-memory offset in every CTA of `cta_mask` (bit r = cluster rank r), and each of those
+// CTAs' mbarrier at the offset of `bar` receives the complete_tx of the bytes written into that CTA.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;"
+      ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask), "l"(hint)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1,

@@ -10,6 +10,12 @@
 //
 // The producer runs ahead into the next tile of the persistent loop while the MMA warpgroups are in their epilogue.
 // A and W are both K-major ("TN" GEMM: nn.Linear weight layout), fp32 accumulation, bf16 output.
+//
+// CLUSTER = 2 (every GEMM with two or more M tiles, not the convolution): the two CTAs of a cluster compute M tiles
+// 2i and 2i + 1 of the same N tile, so they need the same W tile. Each producer loads its own A tile and one half
+// (BN / 2 rows) of W, multicast into the same place of the stage in both CTAs: per K block a CTA reads 16 KiB of A and
+// BN * 64 B of W from L2 instead of 16 KiB + BN * 128 B. A stage is refilled only when the MMA warps of BOTH CTAs are
+// done with it (each releases it in both CTAs), so the two CTAs walk the same tiles with their rings in lockstep.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -33,37 +39,53 @@ struct GemmCfg {
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-template <int BN, int EPI, bool CONV = false>
+template <int BN, int EPI, bool CONV = false, int CLUSTER = 1>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr int kStages = Cfg::kStages;
   static_assert(EPI != EPI_SWIGLU || BN == 256, "SwiGLU epilogue pairs 128 gate + 128 up columns");
+  static_assert(CLUSTER == 1 || (CLUSTER == 2 && !CONV), "CTA pairs for the plain GEMM only");
+  constexpr int kBSliceRows = BN / CLUSTER;   // W rows one producer loads per stage (tmB's box)
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * Cfg::kABytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
-  uint64_t* full_bar = bars;                  // [kStages]  TMA -> MMA
-  uint64_t* empty_bar = bars + kStages;       // [kStages]  MMA -> TMA (one arrive per MMA warp)
+  uint64_t* full_bar = bars;                  // [kStages]  TMA -> MMA: the local producer's arrive + the stage's bytes
+  uint64_t* empty_bar = bars + kStages;       // [kStages]  MMA -> TMA: one arrive per MMA warp of every CTA of the cluster
 
   const int wg = threadIdx.x >> 7;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_k = CONV ? p.ksize * p.ksize * p.cin_chunks : (p.K + BK - 1) / BK;
+  // persistent loop over cluster tiles (CLUSTER M tiles x one N tile); this CTA takes M tile CLUSTER * m + rank
+  const uint32_t rank = (CLUSTER > 1) ? cluster_ctarank() : 0u;
+  const int num_mc = (p.num_m + CLUSTER - 1) / CLUSTER;
+  const int first_tile = blockIdx.x / CLUSTER, tile_stride = gridDim.x / CLUSTER;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kGemmMmaWarps);
+      mbar_init(&empty_bar[i], CLUSTER * kGemmMmaWarps);
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  if constexpr (CLUSTER > 1) cluster_sync_all();   // the peer's barriers exist before any remote arrive or multicast
+  else __syncthreads();
+
+  // A consumed stage is released (once per MMA warp) in every CTA whose producer writes into it: lane r arrives in rank r.
+  auto release = [&](int s) {
+    if constexpr (CLUSTER == 1) {
+      if (lane == 0) mbar_arrive(&empty_bar[s]);
+    } else if (lane < CLUSTER) {
+      mbar_arrive_cluster(&empty_bar[s], (uint32_t)lane);
+    }
+  };
 
   if (wg == 0) {
     // ===================== TMA producer =====================
@@ -73,9 +95,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       uint32_t phase = 0;
       const uint64_t hint_a = (p.hints & 2) ? kEvictFirst : ((p.hints & 8) ? kEvictLast : kEvictNormal);
       const uint64_t hint_w = (p.hints & 1) ? kEvictLast : ((p.hints & 16) ? kEvictFirst : kEvictNormal);
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      for (int tile = first_tile; tile < p.num_tiles; tile += tile_stride) {
         int m_blk, n_blk;
-        tile_coords(tile, p.num_m, p.num_n, p.group_m, p.group_n, m_blk, n_blk);
+        tile_coords(tile, num_mc, p.num_n, p.group_m, p.group_n, m_blk, n_blk);
+        m_blk = m_blk * CLUSTER + rank;   // past the last M tile (odd count): TMA zero-fills, the epilogue skips the rows
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
@@ -92,7 +115,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           } else {
             tma_load_2d(smem_a + stage * Cfg::kABytes, &tmA, &full_bar[stage], kb * BK, m_blk * BM, hint_a);
           }
-          tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * BK, n_blk * BN, hint_w);
+          // W rows [n_blk * BN + rank * kBSliceRows, + kBSliceRows) into the same rows of the stage in every CTA of the
+          // cluster; 128B-swizzled K-major slices of a multiple of 8 rows put together are byte-identical to one BN-row box
+          uint8_t* b_dst = smem_b + stage * Cfg::kBBytes + rank * (kBSliceRows * BK * 2);
+          const int b_row = n_blk * BN + (int)rank * kBSliceRows;
+          if constexpr (CLUSTER == 1) tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, b_row, hint_w);
+          else tma_load_2d_multicast(b_dst, &tmB, &full_bar[stage], kb * BK, b_row, (1u << CLUSTER) - 1, hint_w);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -104,9 +132,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int wq = warp & 3;                      // warp within the warpgroup: fragment rows 16 wq .. 16 wq + 15
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    for (int tile = first_tile; tile < p.num_tiles; tile += tile_stride) {
       int m_blk, n_blk;
-      tile_coords(tile, p.num_m, p.num_n, p.group_m, p.group_n, m_blk, n_blk);
+      tile_coords(tile, num_mc, p.num_n, p.group_m, p.group_n, m_blk, n_blk);
+      m_blk = m_blk * CLUSTER + rank;
       float acc[BN / 2];
       int prev = 0;
       for (int kb = 0; kb < num_k; ++kb) {
@@ -120,7 +149,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (kb > 0) {   // the previous k block's MMAs have retired: its smem slot may be refilled
           wgmma_wait<1>();
           __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          release(prev);
         }
         prev = stage;
         if (++stage == kStages) { stage = 0; phase ^= 1; }
@@ -128,7 +157,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_wait<0>();
       gmma_fence_operand(acc);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      release(prev);
 
       // epilogue: this thread holds rows r0 = 16 wq + lane / 4 and r0 + 8 (of its 64-row half), columns 8c + 2 (lane % 4) + {0, 1}
       const int cq = 2 * (lane & 3);
@@ -214,53 +243,95 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   }
+
+  if constexpr (CLUSTER > 1) {   // the peer may still arrive on this CTA's empty barriers: leave together
+    __syncwarp();
+    cluster_sync_all();
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <int BN, int EPI, bool CONV = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
+// Cluster size of a (non-convolution) GEMM over M rows: CTA pairs sharing the W tile as soon as there are two M tiles.
+// tmB's box is BN / cluster rows.
+static int gemm_cluster(int M) { return (M + BM - 1) / BM >= 2 ? 2 : 1; }
+
+template <int BN, int EPI, bool CONV, int CLUSTER>
+static int launch_gemm_cluster(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<BN, EPI, CONV>;
-  static bool attr_done = false;  // per-instantiation; idempotent if raced
-  if (!attr_done) {
+  auto kern = gemm_bf16_kernel<BN, EPI, CONV, CLUSTER>;
+  cudaLaunchConfig_t cfg{};
+  cfg.blockDim = dim3(kGemmThreads, 1, 1);
+  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = CLUSTER;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  static int max_ctas = 0;  // per-instantiation; idempotent if raced
+  if (max_ctas == 0) {
     BAGEL_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_done = true;
+    int n = sm_count();
+    if (CLUSTER > 1) {   // how many pairs fit at once depends on how the SMs are spread over the GPCs
+      cfg.gridDim = dim3(CLUSTER, 1, 1);
+      BAGEL_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+      if (n < 1) return set_error(BAGEL_ERR_CUDA, "bagel_gemm_bf16: no %d-CTA cluster fits on this device", CLUSTER);
+      n *= CLUSTER;
+    }
+    max_ctas = n;
   }
   if (!CONV) p.num_m = (p.M + BM - 1) / BM;  // CONV: set by the caller (images x tiles per image)
   p.num_n = (p.N + BN - 1) / BN;
-  p.num_tiles = p.num_m * p.num_n;
+  p.num_tiles = (p.num_m + CLUSTER - 1) / CLUSTER * p.num_n;   // cluster tiles
   // Raster group: group_m M-tiles share one sweep over the N tiles: 16 for wide outputs (gate|up: 148 N-tiles), 32 for
-  // narrow ones (14-18 N-tiles: qkv, o_proj, down_proj).
+  // narrow ones (14-18 N-tiles: qkv, o_proj, down_proj). The kernel counts it in cluster tiles.
   {
     static const int env_g = [] { const char* e = getenv("BAGEL_GEMM_GROUP_M"); return e ? atoi(e) : 0; }();
     static const int env_n = [] { const char* e = getenv("BAGEL_GEMM_GROUP_N"); return e ? atoi(e) : -1; }();
     static const int env_h = [] { const char* e = getenv("BAGEL_GEMM_HINTS"); return e ? atoi(e) : -1; }();
-    p.group_m = env_g > 0 ? env_g : (p.num_n >= 64 ? 16 : 32);
+    const int group_m = env_g > 0 ? env_g : (p.num_n >= 64 ? 16 : 32);
+    p.group_m = group_m >= CLUSTER ? group_m / CLUSTER : 1;
     // N super-tiles only where W does not fit the L2 beside the streams (gate|up: 272 MB); 0 / >= num_n = one sweep
     int gn = env_n >= 0 ? env_n : 0;
     if (gn <= 0 || gn > p.num_n) gn = p.num_n;
     p.group_n = gn;
     p.hints = env_h >= 0 ? env_h : 0;
   }
-  const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
-  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(tmA, tmB, p);
+  const int grid = p.num_tiles * CLUSTER < max_ctas ? p.num_tiles * CLUSTER : max_ctas;
+  if (CLUSTER == 1) {
+    kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(tmA, tmB, p);
+  } else {
+    cfg.gridDim = dim3((unsigned)grid, 1, 1);
+    BAGEL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p));
+  }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   BAGEL_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
+template <int BN, int EPI, bool CONV = false>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream,
+                       int cluster) {
+  if constexpr (!CONV) {
+    if (cluster == 2) return launch_gemm_cluster<BN, EPI, CONV, 2>(tmA, tmB, p, stream);
+  }
+  return launch_gemm_cluster<BN, EPI, CONV, 1>(tmA, tmB, p, stream);
+}
+
 template <int BN>
 static int dispatch_epi(int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
-                        cudaStream_t s) {
+                        cudaStream_t s, int cluster) {
   switch (epi) {
-    case EPI_BIAS: return launch_gemm<BN, EPI_BIAS>(tmA, tmB, p, s);
-    case EPI_RESID: return launch_gemm<BN, EPI_RESID>(tmA, tmB, p, s);
-    case EPI_GELU: return launch_gemm<BN, EPI_GELU>(tmA, tmB, p, s);
-    case EPI_SILU: return launch_gemm<BN, EPI_SILU>(tmA, tmB, p, s);
-    case EPI_F32: return launch_gemm<BN, EPI_F32>(tmA, tmB, p, s);
-    case EPI_RESID_F32: return launch_gemm<BN, EPI_RESID_F32>(tmA, tmB, p, s);
+    case EPI_BIAS: return launch_gemm<BN, EPI_BIAS>(tmA, tmB, p, s, cluster);
+    case EPI_RESID: return launch_gemm<BN, EPI_RESID>(tmA, tmB, p, s, cluster);
+    case EPI_GELU: return launch_gemm<BN, EPI_GELU>(tmA, tmB, p, s, cluster);
+    case EPI_SILU: return launch_gemm<BN, EPI_SILU>(tmA, tmB, p, s, cluster);
+    case EPI_F32: return launch_gemm<BN, EPI_F32>(tmA, tmB, p, s, cluster);
+    case EPI_RESID_F32: return launch_gemm<BN, EPI_RESID_F32>(tmA, tmB, p, s, cluster);
     default: return set_error(BAGEL_ERR_ARG, "bagel_gemm_bf16: unknown epilogue %d", epi);
   }
 }
@@ -310,15 +381,16 @@ extern "C" int bagel_gemm_bf16(const void* A, long long lda, const void* W, long
     // 4x more CTAs (and TMA pipelines) on the W matrix
     if (M <= BM && N >= 1024) bn = (N <= 8192) ? 32 : 64;  // >= 112 CTAs on the 3584/4608-wide projections
   }
+  const int cluster = gemm_cluster(M);
   CUtensorMap tmA, tmB;
   if (int rc = make_tmap_2d_bf16(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM)) return rc;
-  if (int rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, bn)) return rc;
+  if (int rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, bn / cluster)) return rc;
 
-  if (epilogue == EPI_SWIGLU) return launch_gemm<256, EPI_SWIGLU>(tmA, tmB, p, s);
-  if (bn == 256) return dispatch_epi<256>(epilogue, tmA, tmB, p, s);
-  if (bn == 128) return dispatch_epi<128>(epilogue, tmA, tmB, p, s);
-  if (bn == 32) return dispatch_epi<32>(epilogue, tmA, tmB, p, s);
-  return dispatch_epi<64>(epilogue, tmA, tmB, p, s);
+  if (epilogue == EPI_SWIGLU) return launch_gemm<256, EPI_SWIGLU>(tmA, tmB, p, s, cluster);
+  if (bn == 256) return dispatch_epi<256>(epilogue, tmA, tmB, p, s, cluster);
+  if (bn == 128) return dispatch_epi<128>(epilogue, tmA, tmB, p, s, cluster);
+  if (bn == 32) return dispatch_epi<32>(epilogue, tmA, tmB, p, s, cluster);
+  return dispatch_epi<64>(epilogue, tmA, tmB, p, s, cluster);
 }
 
 
@@ -364,9 +436,9 @@ extern "C" int bagel_conv2d_nhwc_bf16(const void* x, int B, int Hi, int Wi, int 
   const int bn = (Cout % 256 == 0 || Cout >= 1024) ? 256 : (Cout > 64 ? 128 : 64);
   if (int rc = make_tmap_2d_bf16(&tmB, w, (uint64_t)p.K, (uint64_t)Cout, (uint64_t)p.K, BK, bn)) return rc;
   const bool res = resid != nullptr;
-  if (bn == 256) return res ? launch_gemm<256, EPI_RESID, true>(tmA, tmB, p, s) : launch_gemm<256, EPI_BIAS, true>(tmA, tmB, p, s);
-  if (bn == 128) return res ? launch_gemm<128, EPI_RESID, true>(tmA, tmB, p, s) : launch_gemm<128, EPI_BIAS, true>(tmA, tmB, p, s);
-  return res ? launch_gemm<64, EPI_RESID, true>(tmA, tmB, p, s) : launch_gemm<64, EPI_BIAS, true>(tmA, tmB, p, s);
+  if (bn == 256) return res ? launch_gemm<256, EPI_RESID, true>(tmA, tmB, p, s, 1) : launch_gemm<256, EPI_BIAS, true>(tmA, tmB, p, s, 1);
+  if (bn == 128) return res ? launch_gemm<128, EPI_RESID, true>(tmA, tmB, p, s, 1) : launch_gemm<128, EPI_BIAS, true>(tmA, tmB, p, s, 1);
+  return res ? launch_gemm<64, EPI_RESID, true>(tmA, tmB, p, s, 1) : launch_gemm<64, EPI_BIAS, true>(tmA, tmB, p, s, 1);
 }
 
 
@@ -400,8 +472,9 @@ extern "C" int bagel_gemm_qkv_norm_rope(const void* A, long long lda, const void
   p.qkv.v_out = static_cast<__nv_bfloat16*>(v_out);
   p.qkv.ld_q = ld_q; p.qkv.ld_kv = ld_kv; p.qkv.kv_rows = kv_rows;
   p.qkv.Hq = Hq; p.qkv.Hk = Hk; p.qkv.eps = eps; p.qkv.fp32_flow = fp32_flow;
+  const int cluster = gemm_cluster(M);
   CUtensorMap tmA, tmB;
   if (int rc = make_tmap_2d_bf16(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM)) return rc;
-  if (int rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, 256)) return rc;
-  return launch_gemm<256, EPI_QKV>(tmA, tmB, p, static_cast<cudaStream_t>(stream));
+  if (int rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BK, 256 / cluster)) return rc;
+  return launch_gemm<256, EPI_QKV>(tmA, tmB, p, static_cast<cudaStream_t>(stream), cluster);
 }

@@ -45,22 +45,6 @@ __device__ __forceinline__ float gelu_tanh_s(float x) {
 }
 __device__ __forceinline__ float silu_s(float x) { return x / (1.0f + __expf(-x)); }
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ float ld_dsmem_f32(uint32_t local_addr, uint32_t rank) {
-  uint32_t remote;
-  float v;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local_addr), "r"(rank));
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
-  return v;
-}
 // the 128 threads of the MMA warpgroup only
 __device__ __forceinline__ void mma_wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
