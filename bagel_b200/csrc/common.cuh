@@ -61,13 +61,18 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a protocol bug must surface as a trap (-> cudaErrorLaunchFailure on the host), never as a
 // hung GPU. ~4e9 cycles is seconds of wall clock, far beyond any legitimate wait in these kernels.
+// The diagnostic message is a debug build only (-DBAGEL_MBAR_TRACE, see tools/build_variant.py): printf is a call
+// (vprintf), and a call anywhere on a path that runs while a wgmma group is in flight makes ptxas serialize every
+// wgmma of the kernel (C7510 "wgmma pipeline crossing function boundary").
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > 4000000000LL) {
+#ifdef BAGEL_MBAR_TRACE
       printf("bagel_b200: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n", blockIdx.x,
              threadIdx.x, smem_u32(bar), parity);
+#endif
       __trap();
     }
   }
