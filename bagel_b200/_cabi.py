@@ -25,6 +25,8 @@ SIGNATURES = {
     "bagel_abi_version": (_i, []),
     "bagel_launch_count": (_ll, []),
     "bagel_gemm_bf16": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _vp, _ll, _vp, _i, _vp]),
+    "bagel_quantize_fp8_bf16": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp]),
+    "bagel_gemm_fp8": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _ll, _i, _i, _i, _vp, _ll, _i, _vp]),
     "bagel_gemm_qkv_norm_rope": (_i, [_vp, _ll, _vp, _ll, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll,
                                       _vp, _vp, _ll, _vp, _i, _i, _f, _i, _vp]),
     "bagel_attn_varlen_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f,

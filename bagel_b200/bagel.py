@@ -106,6 +106,8 @@ class Bagel:
         self.device = language_model.device
         # "A": bf16 weights + autocast (app.py:111); "B": fp32 master weights + autocast (eval drivers) — see qwen2_navit.py
         self.dtype_mode = language_model.model.dtype_mode
+        # opt-in block-scaled FP8 MLP of the generation expert (inference only; bagel_b200/fp8.py)
+        self.fp8_gen_mlp = language_model.model.fp8_gen_mlp
         sdt = language_model.model.stream_dtype
         llm = config.llm_config
         self.hidden_size = llm.hidden_size
@@ -686,6 +688,9 @@ class Bagel:
                                       "cannot be mapped onto the varlen attention kernel)")
         if self.dtype_mode != "A":
             raise NotImplementedError("Bagel.forward is implemented for dtype_mode='A'")
+        if self.fp8_gen_mlp:
+            raise NotImplementedError("Bagel.forward (training numerics) is not implemented with fp8_gen_mlp=True, which "
+                                      "is an inference mode: load the model with fp8_gen_mlp=False")
         dev = self.device
         lm = self.language_model.model
         L = int(sequence_length)

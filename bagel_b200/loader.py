@@ -42,11 +42,13 @@ def read_safetensors(path: str) -> Dict[str, torch.Tensor]:
 
 
 def load_bagel(model_path: str, device="cuda", max_latent_size: int = 64,
-               state_dict: Optional[Dict[str, torch.Tensor]] = None, dtype_mode: str = "A") -> Tuple[Bagel, AutoEncoder, BagelConfig]:
+               state_dict: Optional[Dict[str, torch.Tensor]] = None, dtype_mode: str = "A",
+               fp8_gen_mlp: bool = False) -> Tuple[Bagel, AutoEncoder, BagelConfig]:
     """Returns (model, vae_model, config) ready for InterleaveInferencer(model, vae_model, tokenizer, ...).
-    dtype_mode "A": checkpoint cast to bf16 (app.py:111); "B": fp32 master weights + autocast numerics (eval drivers)."""
+    dtype_mode "A": checkpoint cast to bf16 (app.py:111); "B": fp32 master weights + autocast numerics (eval drivers).
+    fp8_gen_mlp=True: the generation expert's gate/up/down_proj are quantised to block-scaled FP8 at load (bagel_b200/fp8.py)."""
     cfg = load_configs(model_path, max_latent_size)
-    lm = Qwen2ForCausalLM(cfg.llm_config, device=device, dtype_mode=dtype_mode)
+    lm = Qwen2ForCausalLM(cfg.llm_config, device=device, dtype_mode=dtype_mode, fp8_gen_mlp=fp8_gen_mlp)
     vit = SiglipVisionModel(cfg.vit_config, device=device)
     model = Bagel(lm, vit, cfg)
     sd = state_dict if state_dict is not None else read_safetensors(os.path.join(model_path, "ema.safetensors"))

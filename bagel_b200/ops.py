@@ -104,6 +104,61 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, bias: Optional[torch.Tensor] = Non
     return out
 
 
+FP8 = torch.float8_e4m3fn
+
+
+def quantize_fp8(x: torch.Tensor, block_rows: int = 1, *, q: Optional[torch.Tensor] = None,
+                 scales: Optional[torch.Tensor] = None):
+    """Block-scaled e4m3 quantisation of a bf16 [M, K] tensor (K % 128 == 0): returns (q [M, K] float8_e4m3fn,
+    fp32 power-of-two scales). block_rows=1: one scale per 1 x 128 group, K-block major [K/128, M] (activations);
+    block_rows=128: one per 128 x 128 block, [ceil(M/128), K/128] (weights). See bagel_quantize_fp8_bf16."""
+    _req(x, torch.bfloat16, "x")
+    M, K = x.shape
+    if q is None:
+        q = torch.empty((M, K), dtype=FP8, device=x.device)
+    _req(q, FP8, "q")
+    assert q.shape == (M, K)
+    shape = (K // 128, M) if block_rows == 1 else ((M + 127) // 128, K // 128)
+    if scales is None:
+        scales = torch.empty(shape, dtype=torch.float32, device=x.device)
+    _req(scales, torch.float32, "scales")
+    assert scales.dim() == 2 and scales.shape[0] == shape[0] and scales.shape[1] >= shape[1]
+    rc = _cabi.lib().bagel_quantize_fp8_bf16(_ptr(x), x.stride(0), _ptr(q), q.stride(0), _ptr(scales), scales.stride(0),
+                                             M, K, int(block_rows), _stream())
+    _cabi.check(rc, "bagel_quantize_fp8_bf16")
+    return q, scales
+
+
+def gemm_fp8(a: torch.Tensor, a_scales: torch.Tensor, w: torch.Tensor, w_scales: torch.Tensor, *,
+             resid: Optional[torch.Tensor] = None, epilogue: int = EPI_RESID,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out = epilogue(dequant(a) @ dequant(w).T) with block-scaled e4m3 operands: a [M, K] with a_scales [K/128, >= M]
+    (quantize_fp8 block_rows=1), w [N, K] with w_scales [N/64, K/128] (see bagel_b200.fp8 for the weight layouts).
+    EPI_SWIGLU (w gate|up interleaved per 64 rows, out [M, N/2]) or EPI_RESID (out [M, N] = resid + y)."""
+    _req(a, FP8, "a")
+    _req(w, FP8, "w")
+    _req(a_scales, torch.float32, "a_scales")
+    _req(w_scales, torch.float32, "w_scales")
+    M, K = a.shape
+    N = w.shape[0]
+    assert w.shape[1] == K and w_scales.is_contiguous() and w_scales.shape == (N // 64, K // 128)
+    assert a_scales.shape[0] == K // 128 and a_scales.shape[1] >= M
+    n_out = N // 2 if epilogue == EPI_SWIGLU else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=torch.bfloat16, device=a.device)
+    _req(out, torch.bfloat16, "out")
+    assert out.shape[1] == n_out
+    ldr = 0
+    if resid is not None:
+        _req(resid, torch.bfloat16, "resid")
+        ldr = resid.stride(0)
+    rc = _cabi.lib().bagel_gemm_fp8(_ptr(a), a.stride(0), _ptr(a_scales), a_scales.stride(0), _ptr(w), w.stride(0),
+                                    _ptr(w_scales), _ptr(out), out.stride(0), M, N, K, _ptr(resid), ldr, epilogue,
+                                    _stream())
+    _cabi.check(rc, "bagel_gemm_fp8")
+    return out
+
+
 def gemm_qkv_norm_rope(a, w, bias, q_w0, k_w0, q_w1, k_w1, expert, cos, sin, q_out, k_out, v_out, kv_rows, Hq, Hk,
                        eps: float, fp32_flow: bool, row_map=None):
     """Fused QKV projection + per-head q/k RMSNorm + RoPE + bf16 cast + K/V placement (head_dim 128)."""

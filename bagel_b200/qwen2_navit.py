@@ -24,6 +24,7 @@ from typing import Dict, List, Optional
 
 import torch
 
+from . import fp8 as _fp8
 from . import ops
 from .config import Qwen2Config
 
@@ -91,7 +92,8 @@ class _Linear:
 
 class _ExpertWeights:
     """One expert's ("" = und, "_moe_gen" = gen) weights of one decoder layer, in kernel layouts."""
-    __slots__ = ("wqkv", "bqkv", "wo", "wgu", "wd", "ln_in", "ln_post", "q_norm", "k_norm")
+    __slots__ = ("wqkv", "bqkv", "wo", "wgu", "wd", "ln_in", "ln_post", "q_norm", "k_norm", "fp8")
+    # fp8: the gen expert's MLP as bagel_b200.fp8.GenMlpFp8 when the model has fp8_gen_mlp=True (wgu / wd are then None)
 
 
 class _Layer:
@@ -192,7 +194,7 @@ class ForwardPlan:
 class Qwen2Model:
     """The decoder stack (reference Qwen2Model, qwen2_navit.py:943-1092)."""
 
-    def __init__(self, config: Qwen2Config, device="cuda", dtype_mode: str = "A"):
+    def __init__(self, config: Qwen2Config, device="cuda", dtype_mode: str = "A", fp8_gen_mlp: bool = False):
         self.config = config
         self.device = torch.device(device)
         if dtype_mode not in ("A", "B"):
@@ -205,6 +207,16 @@ class Qwen2Model:
             raise ValueError(f"unknown layer_module {config.layer_module!r}; expected one of {sorted(kinds)}")
         self.layer_kind = kinds[config.layer_module]
         self.use_moe = "Mo" in config.layer_module      # same test as the reference (:948): MoE and MoT
+        # opt-in block-scaled FP8 gate/up/down of the generation expert (bagel_b200/fp8.py); everything else stays mode A
+        self.fp8_gen_mlp = bool(fp8_gen_mlp)
+        if self.fp8_gen_mlp:
+            if dtype_mode != "A":
+                raise NotImplementedError("fp8_gen_mlp=True is implemented for dtype_mode='A' (bf16 residual stream)")
+            if not self.use_moe:
+                raise ValueError(f"fp8_gen_mlp=True needs a generation expert (mlp_moe_gen); {config.layer_module} has none")
+            if config.hidden_size % 128 or config.intermediate_size % 128:
+                raise ValueError("fp8_gen_mlp=True needs hidden_size and intermediate_size to be multiples of 128 "
+                                 f"(got {config.hidden_size}, {config.intermediate_size})")
         self.enable_taylorseer = False
         self.layers: List[_Layer] = [_Layer() for _ in range(config.num_hidden_layers)]
         self.embed_tokens: Optional[_Embedding] = None
@@ -239,6 +251,23 @@ class Qwen2Model:
         if text_rows:
             for name, cols in (("h_text", H), ("att_text", Hq * D), ("act_text", I)):
                 self._buf(name, text_rows, cols)
+        if self.fp8_gen_mlp:
+            self._fp8_bufs(rows)
+
+    def _scales_buf(self, name: str, groups: int, rows: int) -> torch.Tensor:
+        """Grow-only fp32 [groups, >= rows] buffer of K-block-major activation scales (leading dimension = capacity)."""
+        t = self._ws.get(name)
+        if t is None or t.shape[1] < rows or t.shape[0] != groups:
+            t = torch.empty((groups, rows), dtype=torch.float32, device=self.device)
+            self._ws[name] = t
+            self._ws_gen += 1
+        return t
+
+    def _fp8_bufs(self, rows: int):
+        """e4m3 copies of the MLP block's two GEMM inputs (h, act) and their scales."""
+        H, I = self.config.hidden_size, self.config.intermediate_size
+        return (self._buf("h_fp8", rows, H, ops.FP8), self._scales_buf("h_fp8_s", H // 128, rows),
+                self._buf("act_fp8", rows, I, ops.FP8), self._scales_buf("act_fp8_s", I // 128, rows))
 
     def alloc_kv(self, plan: ForwardPlan):
         """Merged K/V buffers [total_kv, Hk*D] for every layer (the reference re-allocates these per layer per
@@ -289,6 +318,9 @@ class Qwen2Model:
         q = self._buf("q", n, Hq * D)
         att = self._buf("att", n, Hq * D)
         act = self._buf("act", n, I)
+        fp8 = routed and self.fp8_gen_mlp     # the gen rows' MLP in block-scaled FP8
+        if fp8:
+            hq, hs, aq, as_ = self._fp8_bufs(n)
         if nt:
             ht = self._buf("h_text", nt, H)
             at = self._buf("att_text", nt, Hq * D)
@@ -328,8 +360,14 @@ class Qwen2Model:
                 ops.gemm(at, und.wo, resid=xa, row_map=plan.text_rows, epilogue=EPI_R, out=xb)
             # ---- MLP block ----
             rmsnorm(xb, und.ln_post, amain.ln_post if a_routed else None, a_expert, eps, out=h)
-            ops.gemm(h, main.wgu, epilogue=ops.EPI_SWIGLU, out=act)
-            ops.gemm(act, main.wd, resid=xb, epilogue=EPI_R, out=xa)
+            if fp8:
+                ops.quantize_fp8(h, 1, q=hq, scales=hs)
+                ops.gemm_fp8(hq, hs, main.fp8.wgu, main.fp8.wgu_s, epilogue=ops.EPI_SWIGLU, out=act)
+                ops.quantize_fp8(act, 1, q=aq, scales=as_)
+                ops.gemm_fp8(aq, as_, main.fp8.wd, main.fp8.wd_s, resid=xb, epilogue=ops.EPI_RESID, out=xa)
+            else:
+                ops.gemm(h, main.wgu, epilogue=ops.EPI_SWIGLU, out=act)
+                ops.gemm(act, main.wd, resid=xb, epilogue=EPI_R, out=xa)
             if nt:
                 ops.copy_rows(h, ht, src_rows=plan.text_rows)
                 ops.gemm(ht, und.wgu, epilogue=ops.EPI_SWIGLU, out=actt)
@@ -387,9 +425,9 @@ class Qwen2Model:
 class Qwen2ForCausalLM:
     """Reference Qwen2ForCausalLM (qwen2_navit.py:1095-1188): `.model`, `.lm_head`, forward_inference(...)."""
 
-    def __init__(self, config: Qwen2Config, device="cuda", dtype_mode: str = "A"):
+    def __init__(self, config: Qwen2Config, device="cuda", dtype_mode: str = "A", fp8_gen_mlp: bool = False):
         self.config = config
-        self.model = Qwen2Model(config, device, dtype_mode)
+        self.model = Qwen2Model(config, device, dtype_mode, fp8_gen_mlp)
         self.lm_head: Optional[_Linear] = None
         self.vocab_size = config.vocab_size
 
@@ -423,6 +461,17 @@ class Qwen2ForCausalLM:
                 raise KeyError(f"missing weight {name}")
             return None
 
+        def load_mlp(e: _ExpertWeights, m: str, gen: bool):
+            if gen and self.model.fp8_gen_mlp:
+                # quantised from the bf16 matrices, which are dropped afterwards: only the e4m3 copies stay on the device
+                e.fp8 = _fp8.GenMlpFp8.from_reference(get(m + "gate_proj.weight"), get(m + "up_proj.weight"),
+                                                      get(m + "down_proj.weight"))
+                e.wgu = e.wd = None
+            else:
+                e.wgu = ops.interleave_gate_up(get(m + "gate_proj.weight"), get(m + "up_proj.weight"))
+                e.wd = get(m + "down_proj.weight").contiguous()
+                e.fp8 = None
+
         self.model.embed_tokens = _Embedding(get("model.embed_tokens.weight", dtype=sdt).contiguous())
         for li, layer in enumerate(self.model.layers):
             p = f"model.layers.{li}."
@@ -432,9 +481,7 @@ class Qwen2ForCausalLM:
                 e = _ExpertWeights()
                 if sfx and self.model.layer_kind == "moe":
                     # Qwen2MoEDecoderLayer: only the MLP is duplicated (mlp_moe_gen); attention / norms are shared
-                    m = p + f"mlp{sfx}."
-                    e.wgu = ops.interleave_gate_up(get(m + "gate_proj.weight"), get(m + "up_proj.weight"))
-                    e.wd = get(m + "down_proj.weight").contiguous()
+                    load_mlp(e, p + f"mlp{sfx}.", bool(sfx))
                     u = layer.und
                     e.wqkv, e.bqkv, e.wo, e.ln_in, e.ln_post, e.q_norm, e.k_norm = (u.wqkv, u.bqkv, u.wo, u.ln_in,
                                                                                      u.ln_post, u.q_norm, u.k_norm)
@@ -454,9 +501,7 @@ class Qwen2ForCausalLM:
                     # QKV epilogue has no norm-free variant, so say so at load time instead of mis-computing later
                     raise NotImplementedError("bagel_b200: qk_norm=False is not implemented (every shipped BAGEL loader "
                                               "forces qk_norm=True, app.py:41)")
-                m = p + f"mlp{sfx}."
-                e.wgu = ops.interleave_gate_up(get(m + "gate_proj.weight"), get(m + "up_proj.weight"))
-                e.wd = get(m + "down_proj.weight").contiguous()
+                load_mlp(e, p + f"mlp{sfx}.", bool(sfx))
                 e.ln_in = get(p + f"input_layernorm{sfx}.weight", dtype=sdt).contiguous()
                 e.ln_post = get(p + f"post_attention_layernorm{sfx}.weight", dtype=sdt).contiguous()
                 setattr(layer, tgt, e)

@@ -12,6 +12,7 @@ import torch
 
 from .bagel import Bagel
 from .config import AutoEncoderParams, BagelConfig, Qwen2Config
+from .fp8 import GenMlpFp8
 from .qwen2_navit import Qwen2ForCausalLM, _Embedding, _ExpertWeights, _Linear
 
 BF16 = torch.bfloat16
@@ -41,16 +42,17 @@ def _randn(shape, std, gen, device):
 
 
 def build_random_bagel(llm_kwargs: Dict = None, device="cuda", seed: int = 0, max_latent_size: int = 64,
-                       num_layers: int = None) -> Bagel:
+                       num_layers: int = None, fp8_gen_mlp: bool = False) -> Bagel:
     """Random-init MoT model directly in the kernels' fused layouts (no intermediate fp32 state dict: the 7B
-    model is 28 GB in bf16)."""
+    model is 28 GB in bf16). fp8_gen_mlp=True draws the same weights and quantises the gen expert's MLP layer by
+    layer (bagel_b200/fp8.py), so only its e4m3 copy stays on the device."""
     kw = dict(BAGEL_7B_LLM if llm_kwargs is None else llm_kwargs)
     if num_layers is not None:
         kw["num_hidden_layers"] = num_layers
     llm = Qwen2Config(**kw)
     bcfg = BagelConfig(visual_gen=True, visual_und=False, llm_config=llm, vit_config=None,
                        vae_config=AutoEncoderParams(), latent_patch_size=2, max_latent_size=max_latent_size)
-    lm = Qwen2ForCausalLM(llm, device=device)
+    lm = Qwen2ForCausalLM(llm, device=device, fp8_gen_mlp=fp8_gen_mlp)
     dev = lm.device
     g = torch.Generator(device=dev).manual_seed(seed)
     std = llm.initializer_range
@@ -69,6 +71,10 @@ def build_random_bagel(llm_kwargs: Dict = None, device="cuda", seed: int = 0, ma
             e.ln_post = (1.0 + _randn((H,), 0.02, g, dev).float()).to(BF16)
             e.q_norm = (1.0 + _randn((d,), 0.02, g, dev).float()).to(BF16)
             e.k_norm = (1.0 + _randn((d,), 0.02, g, dev).float()).to(BF16)
+            e.fp8 = None
+            if tgt == "gen" and fp8_gen_mlp:
+                e.fp8 = GenMlpFp8.from_interleaved_bf16(e.wgu, e.wd)
+                e.wgu = e.wd = None
             setattr(layer, tgt, e)
     lm.model.norm = (1.0 + _randn((H,), 0.02, g, dev).float()).to(BF16)
     lm.model.norm_moe_gen = (1.0 + _randn((H,), 0.02, g, dev).float()).to(BF16)

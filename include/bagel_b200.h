@@ -66,6 +66,34 @@ int bagel_gemm_bf16(const void* A, long long lda, const void* W, long long ldw, 
                     int N, int K, const void* bias, const void* resid, long long ldr, const int* row_map,
                     int epilogue, void* stream);
 
+/* Block-scaled FP8 (float8_e4m3fn) quantiser, the opt-in FP8 path of the generation expert's MLP.
+ * X bf16 [M, K] -> Q e4m3 [M, K] (one byte per value, leading dimension ldq in bytes) + fp32 scales. A group is
+ * 1 x 128 values along K (block_rows = 1, activations) or 128 x 128 (block_rows = 128, weights). Each group's scale s is
+ * the smallest power of two with amax <= 448 s, at least 2^-126, and 1 for an all-zero group; Q = e4m3(X / s), round to
+ * nearest even. s is a power of two, so X / s is exact and Q * s is exactly a bf16 value.
+ * Scale layouts:
+ *   block_rows = 1    K-block major: scales[kb * lds + m] for row m and columns [128 kb, 128 kb + 128); lds >= M.
+ *   block_rows = 128  scales[(m / 128) * lds + kb]; lds >= K / 128.
+ * K % 128 == 0, ldx % 8 == 0, ldq % 16 == 0, X and Q 16-byte aligned; ldx, ldq >= K (BAGEL_ERR_ARG otherwise). */
+int bagel_quantize_fp8_bf16(const void* X, long long ldx, void* Q, long long ldq, float* scales, long long lds, int M,
+                            int K, int block_rows, void* stream);
+
+/* C = epilogue(dequant(A) @ dequant(W)^T) with block-scaled e4m3 operands (see bagel_quantize_fp8_bf16):
+ *   y[m, n] = sum_kb a_scales[kb * ld_as + m] * w_scales[(n / 64) * (K / 128) + kb] * (sum_{k in kb} A[m, k] W[n, k]),
+ * each 128-wide K block's tensor-core sum scaled and added into a separate fp32 accumulator, then the bf16 epilogue:
+ *   BAGEL_EPI_SWIGLU  W [2*I, K] with gate/up rows interleaved in blocks of 64 (rows 128t..128t+63 = gate rows 64t..,
+ *                     next 64 = up rows 64t..); C [M, I] = bf16(bf16(silu(bf16 g)) * bf16 u).
+ *   BAGEL_EPI_RESID   C [M, N] = bf16(resid + bf16(y)), resid [*, ldr] bf16.
+ * A [M, K] e4m3 (lda bytes), a_scales as the block_rows = 1 quantiser writes them (ld_as >= M); W [N, K] e4m3 (ldw
+ * bytes); w_scales fp32 [N / 64, K / 128] row-major: one scale per 64-row half of a 128-row tile and K block (a weight
+ * quantised in 128 x 128 blocks repeats each block's scale for its two halves).
+ * K % 128 == 0 and N % 128 == 0 (BAGEL_ERR_SHAPE); lda, ldw % 16 == 0, ldc, ldr % 8 == 0, A, W, C, resid 16-byte
+ * aligned (BAGEL_ERR_ALIGN); lda, ldw >= K, ldc >= the output width (I or N), ldr >= N, and any other epilogue are
+ * BAGEL_ERR_ARG. No bias, no row_map. */
+int bagel_gemm_fp8(const void* A, long long lda, const float* a_scales, long long ld_as, const void* W, long long ldw,
+                   const float* w_scales, void* C, long long ldc, int M, int N, int K, const void* resid, long long ldr,
+                   int epilogue, void* stream);
+
 /* QKV projection with the whole pre-attention tail fused into the GEMM epilogue (head_dim 128 only):
  *   [q|k|v] = A W^T + bias; per-head RMSNorm of q and k with expert-routed weights; RoPE; bf16 cast; q -> q_out,
  *   k / v -> merged KV buffers at row kv_rows[r]. One launch for bagel_gemm_bf16 + bagel_qk_norm_rope, without the
