@@ -34,6 +34,8 @@ SIGNATURES = {
     "bagel_decode_prepare": (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
     "bagel_argmax_rows_bf16": (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp]),
     "bagel_decode_advance": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    "bagel_sample_rows_bf16": (_i, [_vp, _ll, _i, _i, _f, _vp, _vp, _vp, _vp, _vp]),
+    "bagel_decode_advance_stop": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _ll, _i, _vp]),
     "bagel_rmsnorm_bf16": (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _ll, _i, _i, _f, _vp]),
     "bagel_layernorm_bf16": (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _f, _vp]),
     "bagel_rope_table": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),

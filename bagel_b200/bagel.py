@@ -281,10 +281,19 @@ class Bagel:
     # image understanding context: SigLIP tokens (reference bagel.py:299-415)
     # ------------------------------------------------------------------------------------------
     def prepare_vit_images(self, curr_kvlens, curr_rope, images, transforms, new_token_ids):
+        return self.prepare_vit_image_round(curr_kvlens, curr_rope, list(images), transforms, new_token_ids)
+
+    def prepare_vit_image_round(self, curr_kvlens, curr_rope, images, transforms, new_token_ids):
+        """One image round of a batch of independent requests: images[i] is request i's next image, or None when it
+        has no image in this round (prepare_vit_images is the round in which every request has one). A request with an
+        image gets the same position ids, kv lens and row layout (relative to its block) as prepare_vit_images on that
+        image alone. A request without one contributes zero query tokens: its block holds only its cached rows, carried
+        unchanged, and its kv len and rope position stay."""
         cl = torch.tensor(list(curr_kvlens), dtype=torch.int64)
         rope = torch.tensor(list(curr_rope), dtype=torch.int64)
+        has = torch.tensor([im is not None for im in images], dtype=torch.bool)
         tokens, pos = [], []
-        for image in images:
+        for image in (im for im in images if im is not None):
             if hasattr(transforms, "patches") and hasattr(image, "size") and not torch.is_tensor(image):
                 # device-side image path (transforms.DeviceImageTransform): resize + normalise + patchify on the GPU,
                 # bit-identical to the host path below
@@ -296,19 +305,19 @@ class Bagel:
                 tokens.append(patchify(t, self.vit_patch_size))
             pos.append(self.get_flattened_position_ids(h_, w_, self.vit_patch_size,
                                                        max_num_patches_per_side=self.vit_max_num_patch_per_side))
-        ntok = torch.tensor([x.shape[0] for x in tokens], dtype=torch.int64)
-        ql = ntok + 2
+        ntok = torch.zeros(len(images), dtype=torch.int64)
+        ntok[has] = torch.tensor([x.shape[0] for x in tokens], dtype=torch.int64)
+        ql = torch.where(has, ntok + 2, torch.zeros_like(ntok))
         q_start = torch.cumsum(ql, 0) - ql
         b_start = torch.cumsum(cl + ql, 0) - (cl + ql)
-        B = len(images)
         generation_input = {
-            "packed_text_ids": torch.tensor([new_token_ids["start_of_image"], new_token_ids["end_of_image"]] * B,
+            "packed_text_ids": torch.tensor([new_token_ids["start_of_image"], new_token_ids["end_of_image"]] * len(tokens),
                                             dtype=torch.long),
-            "packed_text_indexes": torch.stack([q_start, q_start + ntok + 1], dim=1).reshape(-1),
-            "vit_token_seqlens": ntok.to(torch.int),
+            "packed_text_indexes": torch.stack([q_start[has], q_start[has] + ntok[has] + 1], dim=1).reshape(-1),
+            "vit_token_seqlens": ntok[has].to(torch.int),
             "packed_vit_tokens": torch.cat(tokens, dim=0),
             "packed_vit_position_ids": torch.cat(pos, dim=0),
-            "packed_vit_token_indexes": _ranges(q_start + 1, ntok),
+            "packed_vit_token_indexes": _ranges(q_start[has] + 1, ntok[has]),
             "packed_position_ids": torch.repeat_interleave(rope, ql),
             "packed_seqlens": ql.to(torch.int),
             "packed_indexes": _ranges(b_start + cl, ql),
@@ -316,28 +325,27 @@ class Bagel:
             "key_values_lens": cl.to(torch.int),
         }
         # an image block shares ONE rope position; the counter then advances by 1 (reference :340-343)
-        return generation_input, (cl + ql).tolist(), (rope + 1).tolist()
+        return generation_input, (cl + ql).tolist(), (rope + has.to(torch.int64)).tolist()
 
-    @torch.no_grad()
-    def forward_cache_update_vit(self, past_key_values: NaiveCache, packed_text_ids, packed_text_indexes,
-                                 packed_vit_tokens, packed_vit_token_indexes, packed_vit_position_ids,
-                                 vit_token_seqlens, packed_position_ids, packed_seqlens, packed_indexes,
-                                 packed_key_value_indexes, key_values_lens):
-        dev = self.device
-        lm = self.language_model.model
-        if self.dtype_mode == "B":
-            raise NotImplementedError("dtype_mode='B' covers the LM, the text / VAE prefills and the sampler; the SigLIP tower "
-                                      "runs its bf16-stream path only (mode A)")
-        n = int(torch.as_tensor(packed_seqlens).sum())
-        seq = torch.zeros((n, self.hidden_size), dtype=BF16, device=dev)
-        emb = lm.embed_tokens(torch.as_tensor(packed_text_ids))
-        ops.copy_rows(emb, seq, dst_rows=torch.as_tensor(packed_text_indexes).to(dev, torch.int32))
+    def _vit_features(self, packed_vit_tokens, packed_vit_position_ids, vit_token_seqlens) -> torch.Tensor:
+        """SigLIP tower (per-image varlen) + connector: [sum tokens, LM hidden] bf16."""
         vl = torch.as_tensor(vit_token_seqlens).to("cpu", torch.int64)
         cu = torch.cat([torch.zeros(1, dtype=torch.int64), vl.cumsum(0)]).to(torch.int32)
         feats = self.vit_model(packed_pixel_values=packed_vit_tokens,
                                packed_flattened_position_ids=packed_vit_position_ids, cu_seqlens=cu,
                                max_seqlen=int(vl.max()))
-        feats = self.connector(feats)
+        return self.connector(feats)
+
+    def _prefill_vit_features(self, past_key_values: NaiveCache, feats, packed_text_ids, packed_text_indexes,
+                              packed_vit_token_indexes, packed_vit_position_ids, packed_position_ids, packed_seqlens,
+                              packed_indexes, packed_key_value_indexes, key_values_lens) -> NaiveCache:
+        """LM prefill of image blocks whose SigLIP + connector features are `feats` (reference :390-410)."""
+        dev = self.device
+        lm = self.language_model.model
+        n = int(torch.as_tensor(packed_seqlens).sum())
+        seq = torch.zeros((n, self.hidden_size), dtype=BF16, device=dev)
+        emb = lm.embed_tokens(torch.as_tensor(packed_text_ids))
+        ops.copy_rows(emb, seq, dst_rows=torch.as_tensor(packed_text_indexes).to(dev, torch.int32))
         # + vit_pos_embed[pos], scattered to the image rows of the packed sequence (reference :390-395)
         ops.latent_embed_add(feats, None, self.vit_pos_embed.pos_embed,
                              torch.as_tensor(packed_vit_position_ids).to(dev, torch.int64).contiguous(), seq,
@@ -348,6 +356,19 @@ class Bagel:
             packed_key_value_indexes=packed_key_value_indexes, key_values_lens=key_values_lens,
             update_past_key_values=True, is_causal=False, mode="und")
         return out.past_key_values
+
+    @torch.no_grad()
+    def forward_cache_update_vit(self, past_key_values: NaiveCache, packed_text_ids, packed_text_indexes,
+                                 packed_vit_tokens, packed_vit_token_indexes, packed_vit_position_ids,
+                                 vit_token_seqlens, packed_position_ids, packed_seqlens, packed_indexes,
+                                 packed_key_value_indexes, key_values_lens):
+        if self.dtype_mode == "B":
+            raise NotImplementedError("dtype_mode='B' covers the LM, the text / VAE prefills and the sampler; the SigLIP tower "
+                                      "runs its bf16-stream path only (mode A)")
+        feats = self._vit_features(packed_vit_tokens, packed_vit_position_ids, vit_token_seqlens)
+        return self._prefill_vit_features(past_key_values, feats, packed_text_ids, packed_text_indexes,
+                                          packed_vit_token_indexes, packed_vit_position_ids, packed_position_ids,
+                                          packed_seqlens, packed_indexes, packed_key_value_indexes, key_values_lens)
 
     # ------------------------------------------------------------------------------------------
     # image editing context: clean VAE latents at t=0 (reference bagel.py:417-550)
@@ -581,6 +602,47 @@ class Bagel:
     # ------------------------------------------------------------------------------------------
     # text decode
     # ------------------------------------------------------------------------------------------
+    def _decode_state(self, past_key_values: Optional[NaiveCache], key_values_lens, packed_start_tokens,
+                      packed_query_position_ids, max_length: int) -> Dict[str, Any]:
+        """Device state of a decode of `max_length` steps and its step body (embedding gather -> `run_layers` on a
+        decode `ForwardPlan` -> final norm -> lm_head into `logits`). Every buffer the body touches is fixed, so the
+        body is graph-replayable."""
+        dev = self.device
+        lm = self.language_model.model
+        cfg = lm.config
+        L, w = cfg.num_hidden_layers, cfg.num_key_value_heads * cfg.head_dim
+        kv = torch.as_tensor(key_values_lens).to("cpu", torch.int64)
+        B = int(kv.numel())
+        plan = ForwardPlan.decode(lm, kv, max_length)
+        # zero-filled, not torch.empty: attention multiplies the masked probabilities (exactly 0) with whatever sits in the
+        # spare rows of a slab — 0 x NaN/Inf garbage would poison the output (the attention kernel fetches whole 128-key
+        # blocks by TMA; only the single-query d=128 kernel clamps its loads to the rows in use)
+        kbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
+        vbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
+        if past_key_values is not None and past_key_values.key_cache[0] is not None and plan.n_ctx:
+            lm.place_context(past_key_values, plan.ctx_rows, kbuf, vbuf)
+        st: Dict[str, Any] = {"B": B}
+        st["seq_len"] = seq_len = kv.to(dev, torch.int32)
+        st["pos"] = pos = torch.as_tensor(packed_query_position_ids).to(dev, torch.int64).clone()
+        st["tokens"] = torch.as_tensor(packed_start_tokens).to(dev, torch.int64).clone()
+        st["tokens32"] = tokens32 = st["tokens"].to(torch.int32)
+        st["history"] = torch.zeros((max_length, B), dtype=torch.int64, device=dev)
+        st["step_dev"] = torch.zeros(1, dtype=torch.int32, device=dev)
+        x = lm._buf("xa", B, cfg.hidden_size)      # run_layers' input workspace: the gather needs no extra copy
+        st["logits"] = logits = torch.empty((B, cfg.vocab_size), dtype=BF16, device=dev)
+        head = self.language_model.lm_head
+
+        def body():
+            """One decode step; every input/output is a fixed device buffer (graph-replayable)."""
+            ops.copy_rows(lm.embed_tokens.weight, x, src_rows=tokens32, M=B)
+            ops.rope_table_into(pos, lm.inv_freq, plan.cos, plan.sin, True)
+            ops.decode_prepare(plan.cu_k, seq_len, plan.q_rows, plan.seqused_k)
+            out = lm.run_layers(x, plan, kbuf, vbuf)     # decoder layers + final norm
+            ops.gemm(out, head.weight, bias=head.bias, out=logits)
+
+        st["body"] = body
+        return st
+
     @torch.no_grad()
     def generate_text(self, past_key_values: NaiveCache, packed_key_value_indexes, key_values_lens,
                       packed_start_tokens, packed_query_position_ids, max_length: int, do_sample: bool = False,
@@ -596,41 +658,17 @@ class Bagel:
         in place, attention reads `seqused_k`) -> final norm -> lm_head -> argmax, captured once as a CUDA graph and
         replayed per token. The only host<->device traffic per step is the 8-byte EOS check the reference also
         performs."""
-        dev = self.device
-        lm = self.language_model.model
         if self.dtype_mode == "B":
             raise NotImplementedError("generate_text: the device-resident decode loop is implemented for dtype_mode='A'")
-        cfg = lm.config
-        L, w = cfg.num_hidden_layers, cfg.num_key_value_heads * cfg.head_dim
-        kv = torch.as_tensor(key_values_lens).to("cpu", torch.int64)
-        B = int(kv.numel())
+        dev = self.device
+        B = int(torch.as_tensor(key_values_lens).numel())
         if max_length <= 0:
             return torch.zeros((0, B), dtype=torch.int64, device=dev)
-        plan = ForwardPlan.decode(lm, kv, max_length)
-        # zero-filled, not torch.empty: attention multiplies the masked probabilities (exactly 0) with whatever sits in the
-        # spare rows of a slab — 0 x NaN/Inf garbage would poison the output (the attention kernel fetches whole 128-key
-        # blocks by TMA; only the single-query d=128 kernel clamps its loads to the rows in use)
-        kbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
-        vbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
-        if past_key_values is not None and past_key_values.key_cache[0] is not None and plan.n_ctx:
-            lm.place_context(past_key_values, plan.ctx_rows, kbuf, vbuf)
-        seq_len = kv.to(dev, torch.int32)
-        pos = torch.as_tensor(packed_query_position_ids).to(dev, torch.int64).clone()
-        tokens = torch.as_tensor(packed_start_tokens).to(dev, torch.int64).clone()
-        tokens32 = tokens.to(torch.int32)
-        history = torch.zeros((max_length, B), dtype=torch.int64, device=dev)
-        step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
-        x = lm._buf("xa", B, cfg.hidden_size)      # run_layers' input workspace: the gather needs no extra copy
-        logits = torch.empty((B, cfg.vocab_size), dtype=BF16, device=dev)
-        head = self.language_model.lm_head
-
-        def body():
-            """One decode step; every input/output is a fixed device buffer (graph-replayable)."""
-            ops.copy_rows(lm.embed_tokens.weight, x, src_rows=tokens32, M=B)
-            ops.rope_table_into(pos, lm.inv_freq, plan.cos, plan.sin, True)
-            ops.decode_prepare(plan.cu_k, seq_len, plan.q_rows, plan.seqused_k)
-            out = lm.run_layers(x, plan, kbuf, vbuf)     # decoder layers + final norm
-            ops.gemm(out, head.weight, bias=head.bias, out=logits)
+        d = self._decode_state(past_key_values, key_values_lens, packed_start_tokens, packed_query_position_ids,
+                               max_length)
+        seq_len, pos, tokens, tokens32, history, step_dev = (d[k] for k in ("seq_len", "pos", "tokens", "tokens32",
+                                                                            "history", "step_dev"))
+        logits, body = d["logits"], d["body"]
 
         def greedy_step():
             body()
@@ -660,6 +698,129 @@ class Bagel:
             if end_token_id is not None and int(tokens[0]) == end_token_id:
                 break
         return history[:steps].clone()
+
+    # unfinished-request count: read every STOP_POLL steps, one read behind, so the host never waits on the step it
+    # just queued; at most 2 * STOP_POLL - 1 steps run after the last request has finished
+    STOP_POLL = 4
+    HISTORY_PAD = -1      # history entry of a finished request (no token id is negative)
+
+    @torch.no_grad()
+    def generate_text_batch(self, past_key_values: NaiveCache, packed_key_value_indexes, key_values_lens,
+                            packed_start_tokens, packed_query_position_ids, max_length: int, do_sample: bool = False,
+                            temperature: float = 1.0, end_token_id: Optional[int] = None,
+                            seeds: Optional[Sequence[int]] = None) -> List[torch.Tensor]:
+        """Decode a batch of independent requests (same inputs as generate_text). Returns one LongTensor per request on
+        the model's device: its tokens from the start token up to, not including, its own `end_token_id`, at most
+        `max_length` of them. A finished request's token, sequence length and position freeze while the others go on.
+
+        Greedy picks the first maximum (argmax_rows); do_sample=True draws from softmax(logits / temperature) on the
+        device (Gumbel-max over Philox4x32-10, ops.sample_rows). Request i's draws are keyed by (seed, i): `seeds=None`
+        takes one 32-bit base seed from torch.default_generator (so torch.manual_seed fixes it) for every request,
+        otherwise request i uses seeds[i]. Either way a step is one CUDA-graph replay (after an eager first step), and
+        the host only reads the device's count of unfinished requests, lagged, to stop early."""
+        if self.dtype_mode == "B":
+            raise NotImplementedError("generate_text_batch: the device-resident decode loop is implemented for dtype_mode='A'")
+        if do_sample and not (0.0 < float(temperature) < float("inf")):
+            raise ValueError("generate_text_batch: do_sample=True needs a finite temperature > 0")
+        dev = self.device
+        B = int(torch.as_tensor(key_values_lens).numel())
+        if max_length <= 0:
+            return [torch.zeros(0, dtype=torch.int64, device=dev) for _ in range(B)]
+        if seeds is None:
+            base = int(torch.randint(0, 2 ** 32, (1,), dtype=torch.int64))
+            seeds = [base] * B
+        elif len(seeds) != B:
+            raise ValueError(f"generate_text_batch: {len(seeds)} seeds for {B} requests")
+        d = self._decode_state(past_key_values, key_values_lens, packed_start_tokens, packed_query_position_ids,
+                               max_length)
+        body, logits, history, step_dev = d["body"], d["logits"], d["history"], d["step_dev"]
+        keys = torch.tensor([(int(sd) & 0xFFFFFFFF) | (i << 32) for i, sd in enumerate(seeds)], dtype=torch.int64,
+                            device=dev)
+        nxt = torch.empty(B, dtype=torch.int64, device=dev)
+        finished = torch.zeros(B, dtype=torch.int32, device=dev)
+        unfinished = torch.full((1,), B, dtype=torch.int32, device=dev)
+
+        def step_fn():
+            body()
+            if do_sample:
+                ops.sample_rows(logits, temperature, keys, step_dev, nxt)
+            else:
+                ops.argmax_rows(logits, nxt)
+            ops.decode_advance_stop(d["seq_len"], d["pos"], d["tokens"], d["tokens32"], nxt, history, step_dev, finished,
+                                    unfinished, end_token_id, self.HISTORY_PAD)
+
+        count_host = torch.zeros(2, dtype=torch.int32, pin_memory=True)
+        pending = None        # (event, slot) of the last count copy not yet read
+        graph = None
+        steps = 0
+        for step in range(max_length):
+            if graph is not None:
+                graph.replay()
+            elif step == 1 and self.use_cuda_graph:
+                # step 0 ran eagerly and sized every LM workspace the step uses, so the capture allocates none
+                graph = _capture_graph(step_fn, "the batched decode step")
+                if graph is None:
+                    step_fn()
+            else:
+                step_fn()
+            steps += 1
+            if end_token_id is not None and steps % self.STOP_POLL == 0:
+                slot = (steps // self.STOP_POLL) % 2
+                count_host[slot:slot + 1].copy_(unfinished, non_blocking=True)
+                ev = torch.cuda.Event()
+                ev.record()
+                if pending is not None:
+                    pending[0].synchronize()
+                    if int(count_host[pending[1]]) == 0:
+                        break
+                pending = (ev, slot)
+        hist = history[:steps]
+        lens = (hist != self.HISTORY_PAD).sum(0).tolist()
+        return [hist[:n, i].clone() for i, n in enumerate(lens)]
+
+    @torch.no_grad()
+    def chat_batch(self, tokenizer, new_token_ids, image_transform, requests: Sequence[Tuple[Sequence[Any], str]],
+                   max_length: int, do_sample: bool = False, temperature: float = 1.0,
+                   seeds: Optional[Sequence[int]] = None) -> List[str]:
+        """`chat` for a batch of independent requests, each `(images, prompt)` with any number of images (zero
+        included); returns one answer per request, cut at its own <|im_end|> as `chat` does.
+
+        The context is built as `chat` builds it for each request on its own: image r of a request attends to its
+        images before r, never to later ones or to other requests. One SigLIP call covers every image of every
+        request; then one LM prefill per image round r holds the r-th image of every request that has one (the others
+        take part with no query tokens and their cached rows carried unchanged); then one prefill of all prompts and
+        one `generate_text_batch`."""
+        if self.dtype_mode == "B":
+            raise NotImplementedError("chat_batch: the SigLIP prefill and the decode loop are implemented for dtype_mode='A'")
+        images = [list(imgs) for imgs, _ in requests]
+        R = len(requests)
+        newlens, new_rope = [0] * R, [0] * R
+        rounds = []
+        for r in range(max((len(x) for x in images), default=0)):
+            gi, newlens, new_rope = self.prepare_vit_image_round(
+                newlens, new_rope, [x[r] if r < len(x) else None for x in images], image_transform, new_token_ids)
+            rounds.append(gi)
+        past_key_values = NaiveCache(self.config.llm_config.num_hidden_layers)
+        if rounds:
+            feats = self._vit_features(torch.cat([gi["packed_vit_tokens"] for gi in rounds], dim=0),
+                                       torch.cat([gi["packed_vit_position_ids"] for gi in rounds], dim=0),
+                                       torch.cat([gi["vit_token_seqlens"] for gi in rounds], dim=0))
+            off = 0
+            for gi in rounds:
+                gi = dict(gi)
+                n = gi.pop("packed_vit_tokens").shape[0]
+                gi.pop("vit_token_seqlens")
+                past_key_values = self._prefill_vit_features(past_key_values, feats[off:off + n], **gi)
+                off += n
+        generation_input, newlens, new_rope = self.prepare_prompts(
+            curr_kvlens=newlens, curr_rope=new_rope, prompts=[p for _, p in requests], tokenizer=tokenizer,
+            new_token_ids=new_token_ids)
+        past_key_values = self.forward_cache_update_text(past_key_values, **generation_input)
+        generation_input = self.prepare_start_tokens(newlens, new_rope, new_token_ids)
+        answers = self.generate_text_batch(
+            past_key_values=past_key_values, max_length=max_length, do_sample=do_sample, temperature=temperature,
+            end_token_id=new_token_ids["eos_token_id"], seeds=seeds, **generation_input)
+        return [tokenizer.decode(t).split("<|im_end|>")[0].split("<|im_start|>")[1] for t in answers]
 
     # ------------------------------------------------------------------------------------------
     # training-mode forward (losses only, no backward): reference Bagel.forward, bagel.py:101-229

@@ -443,6 +443,38 @@ def decode_advance(seq_len, pos, tokens, history, step_dev):
     _cabi.check(rc, "bagel_decode_advance")
 
 
+def sample_rows(logits: torch.Tensor, temperature: float, keys: torch.Tensor, step_dev: torch.Tensor,
+                tokens: torch.Tensor, tokens32: Optional[torch.Tensor] = None):
+    """tokens[b] = a draw from softmax(logits[b] / temperature) (Gumbel-max over Philox4x32-10 uniforms keyed by
+    keys[b] = seed | request_id << 32, counter = (step_dev[0], j / 4)); see include/bagel_b200.h."""
+    _req(logits, torch.bfloat16, "logits"); _req(keys, torch.int64, "keys"); _req(step_dev, torch.int32, "step_dev")
+    _req(tokens, torch.int64, "tokens")
+    _opt(tokens32, torch.int32, "tokens32")
+    B, V = logits.shape
+    assert keys.numel() == tokens.numel() == B and (tokens32 is None or tokens32.numel() == B)
+    rc = _cabi.lib().bagel_sample_rows_bf16(_ptr(logits), logits.stride(0), B, V, float(temperature), _ptr(keys),
+                                            _ptr(step_dev), _ptr(tokens), _ptr(tokens32), _stream())
+    _cabi.check(rc, "bagel_sample_rows_bf16")
+
+
+def decode_advance_stop(seq_len, pos, tokens, tokens32, next_tokens, history, step_dev, finished, unfinished,
+                        end_token_id: Optional[int], pad: int):
+    """Per-request stopping of a batched decode step (history [max_length, B]); see include/bagel_b200.h."""
+    for t, dt, nm in ((seq_len, torch.int32, "seq_len"), (pos, torch.int64, "pos"), (tokens, torch.int64, "tokens"),
+                      (tokens32, torch.int32, "tokens32"), (next_tokens, torch.int64, "next_tokens"),
+                      (history, torch.int64, "history"), (step_dev, torch.int32, "step_dev"),
+                      (finished, torch.int32, "finished"), (unfinished, torch.int32, "unfinished")):
+        _req(t, dt, nm)
+    B = seq_len.numel()
+    assert pos.numel() == tokens.numel() == tokens32.numel() == next_tokens.numel() == finished.numel() == B
+    assert history.dim() == 2 and history.is_contiguous() and history.shape[1] == B
+    rc = _cabi.lib().bagel_decode_advance_stop(_ptr(seq_len), _ptr(pos), _ptr(tokens), _ptr(tokens32), _ptr(next_tokens),
+                                               _ptr(history), _ptr(step_dev), _ptr(finished), _ptr(unfinished),
+                                               -1 if end_token_id is None else int(end_token_id), history.shape[0],
+                                               int(pad), B, _stream())
+    _cabi.check(rc, "bagel_decode_advance_stop")
+
+
 def taylor_update(feature: torch.Tensor, factors: torch.Tensor, n_deriv: int, dist: int, rows: Optional[int] = None):
     """TaylorSeer derivative_approximation (cache_utils/taylorseer.py:12-32) on factor planes [orders, cap_rows, H]
     (in place): plane 0 <- feature, plane i+1 <- bf16(bf16(plane_i_new - plane_i_old) / dist) for i < n_deriv."""

@@ -222,6 +222,25 @@ int bagel_argmax_rows_bf16(const void* logits, long long ld, int B, int V, long 
 int bagel_decode_advance(int* seq_len, long long* pos, const long long* tokens, long long* history, int* step_dev, int B,
                          void* stream);
 
+/* Batched decode of independent requests (Bagel.generate_text_batch); state in device memory, graph-replayable:
+ *   bagel_sample_rows_bf16: tokens[b] = a draw from softmax(logits[b, :] / temperature), by Gumbel-max:
+ *     argmax_j (logit_j / T - log(-log u_j)), ties to the lowest index. u_j comes from Philox4x32-10 with key
+ *     (low, high 32 bits of keys[b]) = (seed, request id) and counter (step_dev[0], j / 4, 0, 0), word j % 4; the 23 top
+ *     bits x of that word give u = (x + 0.5) * 2^-23, exact in fp32 and strictly inside (0, 1). A row's draw depends
+ *     only on its logits, key and the step.
+ *     temperature finite and > 0 (greedy decoding is bagel_argmax_rows_bf16); tokens32 may be NULL.
+ *   bagel_decode_advance_stop: per request b, with step = step_dev[0] and history [max_length, B]:
+ *     finished[b] != 0: history[step, b] = pad; nothing else changes (its token, seq_len and pos stay frozen);
+ *     otherwise history[step, b] = tokens[b], then if next[b] == end_token_id or step + 1 == max_length, finished[b] = 1;
+ *     else seq_len[b] += 1, pos[b] += 1, tokens[b] = tokens32[b] = next[b].
+ *     Then unfinished[0] = number of requests not finished, step_dev[0] += 1. Rows of history at step >= max_length are
+ *     not written. B <= 1024; end_token_id < 0 never matches. */
+int bagel_sample_rows_bf16(const void* logits, long long ld, int B, int V, float temperature, const long long* keys,
+                           const int* step_dev, long long* tokens, int* tokens32, void* stream);
+int bagel_decode_advance_stop(int* seq_len, long long* pos, long long* tokens, int* tokens32, const long long* next,
+                              long long* history, int* step_dev, int* finished, int* unfinished, long long end_token_id,
+                              int max_length, long long pad, int B, void* stream);
+
 /* TaylorSeer step cache (reference modeling/cache_utils/taylorseer.py, enabled by generate_image(enable_taylorseer=True),
  * modeling/bagel/bagel.py:678-684; decoder-layer hooks modeling/bagel/qwen2_navit.py:773-777, 824-829).
  * factors: bf16 planes [order][rows][H], plane_stride elements apart, of the last decoder layer's output.
