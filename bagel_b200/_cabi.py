@@ -44,6 +44,8 @@ SIGNATURES = {
     "bagel_copy_rows_bf16": (_i, [_vp, _ll, _vp, _vp, _ll, _vp, _i, _i, _vp]),
     "bagel_latent_embed_add": (_i, [_vp, _ll, _vp, _vp, _ll, _vp, _vp, _ll, _vp, _i, _i, _vp]),
     "bagel_cfg_euler_step": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp, _i, _i, _f, _f, _f, _i, _f, _vp, _vp]),
+    "bagel_cfg_euler_step_batch": (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                        _vp]),
     "bagel_cast_f32_to_bf16": (_i, [_vp, _vp, _ll, _vp]),
     "bagel_conv2d_nhwc_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     "bagel_groupnorm_workspace_bytes": (_ll, [_i, _i]),

@@ -70,6 +70,110 @@ def _cfg_branches(main, text, img, cfg_text_scale: float, cfg_img_scale: float) 
     return [dict(zip(names, b)) for b in branches]
 
 
+def _branch_counts(cfg_text_scale: Sequence[float], cfg_img_scale: Sequence[float]) -> List[int]:
+    """Per request, the number of LM branches _cfg_branches gives it alone (1 main, 2 + text, 3 + image)."""
+    return [len(_cfg_branches((), (), (), sT, sI)) for sT, sI in zip(cfg_text_scale, cfg_img_scale)]
+
+
+def _flow_batch_layout(packed_seqlens, packed_vae_token_indexes, packed_text_indexes, branches: Sequence[Dict[str, Any]],
+                       members: Sequence[Sequence[int]]) -> Dict[str, Any]:
+    """Host layout of one packed LM call of a batch of independent image requests (Bagel.generate_image_batch).
+
+    branches[b] holds the packed inputs of branch b (0 main, 1 text-dropped, 2 image-dropped) over ALL requests, in
+    the keys of _cfg_branches; members[b] lists the requests that take part in block b (blocks with no member are
+    skipped). Block b holds, request after request, the sample [context rows, query rows] that branch b gives the
+    request alone, shifted to the block's place: its position ids and kv len are the branch's, its query and kv indexes
+    are the branch's minus the request's start in the branch packing plus its start in the merged one. The query rows of
+    all blocks are packed in the same order (block, then request).
+
+    Returns the ForwardPlan inputs (query_lens, position_ids, packed_query_indexes, key_values_lens,
+    packed_key_value_indexes, packed_vae_token_indexes, packed_text_indexes), `ctx`: per block (branch, cache rows,
+    merged rows) of the context K/V to place, `copy`: (main query rows, block query rows) of every query row outside
+    block 0 (the latent-in rows of a request are the same in every branch), `rows`: [n_blocks, M] query row of each
+    latent row in each block (-1: request not in the block), and `samples`: (block, request, merged start, query start)."""
+    i64 = lambda t: torch.as_tensor(t).to("cpu", torch.int64).reshape(-1)
+    ql = i64(packed_seqlens)
+    R = int(ql.numel())
+    cq = torch.cumsum(ql, 0) - ql                       # query start of each request in the main packing
+    vae = i64(packed_vae_token_indexes)
+    txt = i64(packed_text_indexes)
+    ntok = ql - 2
+    seg = torch.repeat_interleave(torch.arange(R), ntok)
+    out: Dict[str, Any] = {k: [] for k in ("query_lens", "position_ids", "packed_query_indexes", "key_values_lens",
+                                           "packed_key_value_indexes", "packed_vae_token_indexes",
+                                           "packed_text_indexes", "ctx", "samples")}
+    rows = []
+    copy_src, copy_dst = [], []
+    row_off = 0        # merged K/V row of the next sample
+    q_off = 0          # query row of the next sample
+    for b, mem in enumerate(members):
+        mem = sorted(int(q) for q in mem)
+        if not mem:
+            rows.append(torch.full((int(ntok.sum()),), -1, dtype=torch.int64))
+            continue
+        br = branches[b]
+        cache = br["past_key_values"]
+        has_ctx = cache is not None and cache.key_cache[0] is not None
+        kl = i64(br["key_values_lens"]) if has_ctx else torch.zeros(R, dtype=torch.int64)
+        base = torch.cumsum(kl + ql, 0) - (kl + ql)     # request start in the branch's own packing
+        ckv = torch.cumsum(kl, 0) - kl                  # its first cache row
+        pos, pq = i64(br["packed_position_ids"]), i64(br["packed_query_indexes"])
+        pkv = i64(br["packed_key_value_indexes"]) if has_ctx else torch.zeros(0, dtype=torch.int64)
+        blk_q = torch.full((R,), -1, dtype=torch.int64)  # query start of each request within this block's rows
+        src_rows, dst_rows = [], []
+        for q in mem:
+            qs = slice(int(cq[q]), int(cq[q] + ql[q]))
+            ks = slice(int(ckv[q]), int(ckv[q] + kl[q]))
+            shift = row_off - int(base[q])
+            out["query_lens"].append(ql[q:q + 1])
+            out["position_ids"].append(pos[qs])
+            out["packed_query_indexes"].append(pq[qs] + shift)
+            out["key_values_lens"].append(kl[q:q + 1])
+            out["packed_key_value_indexes"].append(pkv[ks] + shift)
+            src_rows.append(torch.arange(ks.start, ks.stop))
+            dst_rows.append(pkv[ks] + shift)
+            sel_v = (vae >= qs.start) & (vae < qs.stop)
+            sel_t = (txt >= qs.start) & (txt < qs.stop)
+            out["packed_vae_token_indexes"].append(vae[sel_v] - qs.start + q_off)
+            out["packed_text_indexes"].append(txt[sel_t] - qs.start + q_off)
+            out["samples"].append((b, q, row_off, q_off))
+            blk_q[q] = q_off
+            if b:
+                copy_src.append(torch.arange(qs.start, qs.stop))
+                copy_dst.append(torch.arange(q_off, q_off + int(ql[q])))
+            row_off += int(kl[q] + ql[q])
+            q_off += int(ql[q])
+        if has_ctx:
+            out["ctx"].append((b, torch.cat(src_rows), torch.cat(dst_rows)))
+        r = torch.full((int(ntok.sum()),), -1, dtype=torch.int64)
+        inb = blk_q[seg] >= 0
+        r[inb] = vae[inb] - cq[seg[inb]] + blk_q[seg[inb]]
+        rows.append(r)
+    for k in ("query_lens", "position_ids", "packed_query_indexes", "key_values_lens", "packed_key_value_indexes",
+              "packed_vae_token_indexes", "packed_text_indexes"):
+        out[k] = torch.cat(out[k])
+    cat0 = lambda xs: torch.cat(xs) if xs else torch.zeros(0, dtype=torch.int64)
+    out["copy"] = (cat0(copy_src), cat0(copy_dst))
+    out["rows"] = torch.stack(rows)
+    out["seg"] = seg
+    out["n"] = q_off
+    return out
+
+
+def _flow_batch_schedule(num_timesteps: int, timestep_shift: float, cfg_interval: Sequence[Sequence[float]],
+                         nbs: Sequence[int]):
+    """The shared schedule of a batch and its per-step CFG switches: (ts, dts, cfg_on [steps][R], full [steps]).
+    cfg_on[i][q] is make_flow_runner's test for request q alone; step i runs the all-branch plan when a request that has a
+    text-dropped branch has CFG on."""
+    ts = torch.linspace(1, 0, num_timesteps)
+    ts = timestep_shift * ts / (1 + (timestep_shift - 1) * ts)
+    dts = ts[:-1] - ts[1:]
+    ts = ts[:-1]
+    cfg_on = [[bool(t > iv[0] and t <= iv[1]) for iv in cfg_interval] for t in ts]
+    full = [any(on and nb > 1 for on, nb in zip(row, nbs)) for row in cfg_on]
+    return ts, dts, cfg_on, full
+
+
 def _capture_graph(launch: Callable[[], None], what: str) -> Optional[torch.cuda.CUDAGraph]:
     """Capture launch() as a CUDA graph and replay it once (capture does not execute the work). Capture is an
     optimisation and the eager launch sequence is the same work: on failure, warn, synchronise and return None."""
@@ -208,7 +312,10 @@ class Bagel:
         }
         return generation_input, (cl + tl).tolist(), (rope + tl).tolist()
 
-    def prepare_vae_latent(self, curr_kvlens, curr_rope, image_sizes, new_token_ids):
+    def prepare_vae_latent(self, curr_kvlens, curr_rope, image_sizes, new_token_ids,
+                           generators: Optional[Sequence[torch.Generator]] = None):
+        """generators: optional CPU generator per sample for its init noise (independent requests each with their own
+        seed); by default every sample draws from the global CPU generator, in sample order, like the reference."""
         ds = self.latent_downsample
         cl = torch.tensor(list(curr_kvlens), dtype=torch.int64)
         rope = torch.tensor(list(curr_rope), dtype=torch.int64)
@@ -219,7 +326,10 @@ class Bagel:
         B = len(image_sizes)
         dim = self.latent_channel * self.latent_patch_size ** 2
         # init noise: drawn per sample, in sample order, from the global CPU generator exactly like the reference
-        noises = [torch.randn(int(n), dim) for n in ntok]
+        gens = [None] * B if generators is None else list(generators)
+        if len(gens) != B:
+            raise ValueError(f"prepare_vae_latent: {len(gens)} generators for {B} samples")
+        noises = [torch.randn(int(n), dim, generator=g) for n, g in zip(ntok, gens)]
         pos = [self.get_flattened_position_ids(H, W, ds, max_num_patches_per_side=self.max_latent_size)
                for H, W in image_sizes]
         generation_input = {
@@ -374,16 +484,28 @@ class Bagel:
     # image editing context: clean VAE latents at t=0 (reference bagel.py:417-550)
     # ------------------------------------------------------------------------------------------
     def prepare_vae_images(self, curr_kvlens, curr_rope, images, transforms, new_token_ids, timestep=0):
+        return self.prepare_vae_image_round(curr_kvlens, curr_rope, list(images), transforms, new_token_ids, timestep)
+
+    def prepare_vae_image_round(self, curr_kvlens, curr_rope, images, transforms, new_token_ids, timestep=0,
+                                return_tensors: bool = False):
+        """One VAE image round of a batch of independent requests, with prepare_vit_image_round's contract: images[i] is
+        request i's image or None. A request with an image gets the layout prepare_vae_images gives that image alone; a
+        request without one contributes zero query tokens, keeps its kv len and its rope position. padded_images and
+        patchified_vae_latent_shapes list the present images only, in request order. return_tensors=True also returns
+        the transformed images themselves ([C, H, W] each, present images only), for a caller that encodes them one by
+        one."""
         ds = self.latent_downsample
         cl = torch.tensor(list(curr_kvlens), dtype=torch.int64)
         rope = torch.tensor(list(curr_rope), dtype=torch.int64)
-        tensors = [transforms(im) for im in images]
+        has = torch.tensor([im is not None for im in images], dtype=torch.bool)
+        tensors = [transforms(im) for im in images if im is not None]
         shapes = [(t.shape[1] // ds, t.shape[2] // ds) for t in tensors]
-        ntok = torch.tensor([h * w for h, w in shapes], dtype=torch.int64)
-        ql = ntok + 2
+        ntok = torch.zeros(len(images), dtype=torch.int64)
+        ntok[has] = torch.tensor([h * w for h, w in shapes], dtype=torch.int64)
+        ql = torch.where(has, ntok + 2, torch.zeros_like(ntok))
         q_start = torch.cumsum(ql, 0) - ql
         b_start = torch.cumsum(cl + ql, 0) - (cl + ql)
-        B = len(images)
+        B = len(tensors)
         C = tensors[0].shape[0]
         Hm, Wm = max(t.shape[1] for t in tensors), max(t.shape[2] for t in tensors)
         padded = torch.zeros((B, C, Hm, Wm), device=tensors[0].device)   # stays on the GPU with DeviceImageTransform
@@ -395,23 +517,45 @@ class Bagel:
             "packed_vae_position_ids": torch.cat([self.get_flattened_position_ids(
                 t.size(1), t.size(2), ds, max_num_patches_per_side=self.max_latent_size) for t in tensors], dim=0),
             "packed_timesteps": torch.tensor([timestep]),
-            "packed_vae_token_indexes": _ranges(q_start + 1, ntok),
+            "packed_vae_token_indexes": _ranges(q_start[has] + 1, ntok[has]),
             "packed_text_ids": torch.tensor([new_token_ids["start_of_image"], new_token_ids["end_of_image"]] * B,
                                             dtype=torch.long),
-            "packed_text_indexes": torch.stack([q_start, q_start + ntok + 1], dim=1).reshape(-1),
+            "packed_text_indexes": torch.stack([q_start[has], q_start[has] + ntok[has] + 1], dim=1).reshape(-1),
             "packed_position_ids": torch.repeat_interleave(rope, ql),
             "packed_seqlens": ql.to(torch.int),
             "packed_indexes": _ranges(b_start + cl, ql),
             "packed_key_value_indexes": _ranges(b_start, cl),
             "key_values_lens": cl.to(torch.int),
         }
-        return generation_input, (cl + ql).tolist(), (rope + 1).tolist()
+        out = generation_input, (cl + ql).tolist(), (rope + has.to(torch.int64)).tolist()
+        return (*out, tensors) if return_tensors else out
 
     @torch.no_grad()
     def forward_cache_update_vae(self, vae_model, past_key_values: NaiveCache, padded_images,
                                  patchified_vae_latent_shapes, packed_vae_position_ids, packed_timesteps,
                                  packed_vae_token_indexes, packed_text_ids, packed_text_indexes, packed_position_ids,
                                  packed_seqlens, packed_indexes, key_values_lens, packed_key_value_indexes):
+        latents = vae_model.encode(padded_images)                      # [B, z, Hm/8, Wm/8]
+        return self._prefill_vae_latents(past_key_values, self._patchify_latents(latents, patchified_vae_latent_shapes),
+                                         packed_vae_position_ids, packed_timesteps, packed_vae_token_indexes,
+                                         packed_text_ids, packed_text_indexes, packed_position_ids, packed_seqlens,
+                                         packed_indexes, key_values_lens, packed_key_value_indexes)
+
+    def _patchify_latents(self, latents, patchified_vae_latent_shapes) -> torch.Tensor:
+        """VAE latents [z, >= h*p, >= w*p] each -> packed 2x2-patch rows [sum h*w, p*p*z] bf16, (p, q, c) order
+        (reference :517-518)."""
+        p, zc = self.latent_patch_size, self.latent_channel
+        rows = []
+        for lat, (h, w) in zip(latents, patchified_vae_latent_shapes):
+            lat = lat[:, : h * p, : w * p].reshape(zc, h, p, w, p)
+            rows.append(lat.permute(1, 3, 2, 4, 0).reshape(h * w, p * p * zc))
+        return torch.cat(rows, dim=0).to(self.device, BF16).contiguous()
+
+    def _prefill_vae_latents(self, past_key_values: NaiveCache, packed_latent, packed_vae_position_ids,
+                             packed_timesteps, packed_vae_token_indexes, packed_text_ids, packed_text_indexes,
+                             packed_position_ids, packed_seqlens, packed_indexes, key_values_lens,
+                             packed_key_value_indexes) -> NaiveCache:
+        """LM prefill of clean-latent image blocks whose patchified VAE latents are `packed_latent` (reference :500-550)."""
         dev = self.device
         lm = self.language_model.model
         modeB = self.dtype_mode == "B"
@@ -419,13 +563,6 @@ class Bagel:
         seq = torch.zeros((n, self.hidden_size), dtype=lm.stream_dtype, device=dev)
         emb = lm.embed_tokens(torch.as_tensor(packed_text_ids))
         (ops.copy_rows_f32 if modeB else ops.copy_rows)(emb, seq, dst_rows=torch.as_tensor(packed_text_indexes).to(dev, torch.int32))
-        latents = vae_model.encode(padded_images)                      # [B, z, Hm/8, Wm/8]
-        p, zc = self.latent_patch_size, self.latent_channel
-        rows = []
-        for lat, (h, w) in zip(latents, patchified_vae_latent_shapes):  # 2x2 patchify, (p, q, c) order (:517-518)
-            lat = lat[:, : h * p, : w * p].reshape(zc, h, p, w, p)
-            rows.append(lat.permute(1, 3, 2, 4, 0).reshape(h * w, p * p * zc))
-        packed_latent = torch.cat(rows, dim=0).to(dev, BF16).contiguous()
         proj = ops.gemm(packed_latent, self.vae2llm.weight, bias=self.vae2llm.bias)
         t_emb = self.time_embedder(torch.as_tensor(packed_timesteps).to(dev, torch.float32).reshape(-1)[:1])
         (ops.latent_embed_add_f32 if modeB else ops.latent_embed_add)(
@@ -598,6 +735,127 @@ class Bagel:
         for i in range(runner.num_steps):
             runner.step(i)
         return runner.latents()
+
+    # ------------------------------------------------------------------------------------------
+    # batched image generation of independent requests
+    # ------------------------------------------------------------------------------------------
+    def _build_flow_batch_plan(self, lay: Dict[str, Any], branches: Sequence[Dict[str, Any]]):
+        """ForwardPlan + merged K/V buffers of a _flow_batch_layout, each block's context rows placed from its branch
+        cache (only the member requests' rows), and the device copy map of the latent-in rows outside block 0."""
+        lm = self.language_model.model
+        dev = self.device
+        plan = ForwardPlan(lm, query_lens=lay["query_lens"], position_ids=lay["position_ids"],
+                           packed_query_indexes=lay["packed_query_indexes"], key_values_lens=lay["key_values_lens"],
+                           packed_key_value_indexes=lay["packed_key_value_indexes"], is_causal=False,
+                           mode="gen" if self.use_moe else "und", packed_vae_token_indexes=lay["packed_vae_token_indexes"],
+                           packed_text_indexes=lay["packed_text_indexes"])
+        kbuf, vbuf = lm.alloc_kv(plan)
+        for b, src, dst in lay["ctx"]:
+            if src.numel():
+                lm.place_context(branches[b]["past_key_values"], dst.to(dev, torch.int32), kbuf, vbuf,
+                                 src_rows=src.to(dev, torch.int32))
+        src, dst = lay["copy"]
+        copies = (src.to(dev, torch.int32), dst.to(dev, torch.int32)) if src.numel() else None
+        return plan, kbuf, vbuf, copies
+
+    def _velocity_batch(self, st: Dict[str, Any], key: str, t_row: torch.Tensor, x_src: torch.Tensor):
+        """_velocity + _velocity_head for a batch plan: the latent-in rows are computed once for the main block and
+        copied to the requests' rows in the other blocks (the same values _velocity computes for each branch)."""
+        lm = self.language_model.model
+        plan, kbuf, vbuf, copies = st[key]
+        n = st["n"]
+        seq = lm._buf("xa", plan.n, self.hidden_size, lm.stream_dtype)
+        ops.cast_f32_to_bf16(x_src, out=st["x_bf16"])
+        ops.gemm(st["x_bf16"], self.vae2llm.weight, bias=self.vae2llm.bias, out=st["proj"])
+        ops.latent_embed_add(st["proj"], t_row, self.latent_pos_embed.pos_embed, st["vae_pos"], seq[:n], st["vae_rows"])
+        ops.copy_rows(st["text_emb"], seq[:n], dst_rows=st["text_rows"])
+        if copies is not None:
+            ops.copy_rows(seq, seq, src_rows=copies[0], dst_rows=copies[1])
+        lm.run_layers(seq, plan, kbuf, vbuf, final_norm=False)
+        out = lm.final_norm(plan, for_linear=True)
+        ops.gemm(out, self.llm2vae.weight, bias=self.llm2vae.bias, out=st["v_all"][: plan.n])
+
+    @torch.no_grad()
+    def generate_image_batch(self, packed_text_ids, packed_text_indexes, packed_init_noises, packed_vae_position_ids,
+                             packed_vae_token_indexes, packed_seqlens, packed_position_ids, packed_indexes,
+                             past_key_values: NaiveCache, key_values_lens, packed_key_value_indexes,
+                             cfg_text_scale: Sequence[float], cfg_img_scale: Sequence[float],
+                             cfg_interval: Sequence[Sequence[float]], cfg_renorm_min: Sequence[float],
+                             cfg_renorm_type: Sequence[str], num_timesteps: int = 24, timestep_shift: float = 1.0,
+                             cfg_text_packed_query_indexes=None, cfg_text_packed_position_ids=None,
+                             cfg_text_past_key_values: Optional[NaiveCache] = None, cfg_text_key_values_lens=None,
+                             cfg_text_packed_key_value_indexes=None, cfg_img_packed_query_indexes=None,
+                             cfg_img_packed_position_ids=None, cfg_img_past_key_values: Optional[NaiveCache] = None,
+                             cfg_img_key_values_lens=None, cfg_img_packed_key_value_indexes=None,
+                             enable_taylorseer: bool = False) -> List[torch.Tensor]:
+        """generate_image for R independent requests in one packed denoising run. The packed inputs are those of
+        generate_image over all R samples; cfg_text_scale, cfg_img_scale, cfg_interval, cfg_renorm_min and
+        cfg_renorm_type are per-request lists, num_timesteps and timestep_shift are shared. Returns one [h*w, 64] fp32
+        latent per request.
+
+        Each request gets the branches _cfg_branches gives it alone: the LM call of a step holds a main block with every
+        request, a text-dropped block with the requests that have cfg_text_scale > 1 and an image-dropped block with
+        those that also have cfg_img_scale > 1, each sample attending to its own request's context for that branch. A
+        step runs that all-branch plan when any request with a text-dropped branch has CFG on at its timestep, else the
+        main block alone; bagel_cfg_euler_step_batch then applies each request's own CFG, renorm (a "global" norm covers
+        the request's own rows) and Euler update, with the per-step CFG switch of every request read from a device
+        table, so where FlowRunner captures the step, one graph per plan serves every step."""
+        if enable_taylorseer:
+            raise NotImplementedError("generate_image_batch: TaylorSeer is not implemented for batched requests; use "
+                                      "generate_image(..., enable_taylorseer=True) per request")
+        if self.dtype_mode == "B":
+            raise NotImplementedError("generate_image_batch: the batched sampler is implemented for dtype_mode='A'")
+        dev = self.device
+        ql = torch.as_tensor(packed_seqlens).to("cpu", torch.int64)
+        R = int(ql.numel())
+        per_req = dict(cfg_text_scale=cfg_text_scale, cfg_img_scale=cfg_img_scale, cfg_interval=cfg_interval,
+                       cfg_renorm_min=cfg_renorm_min, cfg_renorm_type=cfg_renorm_type)
+        for k, val in per_req.items():
+            if len(val) != R:
+                raise ValueError(f"generate_image_batch: {k} has {len(val)} entries for {R} requests")
+        for rt in cfg_renorm_type:
+            if rt not in ops.RENORM:
+                raise NotImplementedError(f"{rt} is not supported")
+        nbs = _branch_counts(cfg_text_scale, cfg_img_scale)
+        ts, dts, cfg_on, full = _flow_batch_schedule(num_timesteps, timestep_shift, cfg_interval, nbs)
+        branches = _cfg_branches(
+            (packed_position_ids, packed_indexes, past_key_values, key_values_lens, packed_key_value_indexes),
+            (cfg_text_packed_position_ids, cfg_text_packed_query_indexes, cfg_text_past_key_values,
+             cfg_text_key_values_lens, cfg_text_packed_key_value_indexes),
+            (cfg_img_packed_position_ids, cfg_img_packed_query_indexes, cfg_img_past_key_values,
+             cfg_img_key_values_lens, cfg_img_packed_key_value_indexes), 2.0, 2.0)
+        members = [list(range(R)), [q for q in range(R) if nbs[q] >= 2], [q for q in range(R) if nbs[q] >= 3]]
+        lays = {}
+        if any(full):
+            lays["full"] = _flow_batch_layout(ql, packed_vae_token_indexes, packed_text_indexes, branches, members)
+        if not all(full):
+            lays["main"] = _flow_batch_layout(ql, packed_vae_token_indexes, packed_text_indexes, branches, members[:1])
+        big = lays.get("full", lays.get("main"))
+        # every LM workspace at its final size before the first launch / graph capture (DESIGN §2)
+        self.language_model.model.reserve(big["n"], int(big["packed_text_indexes"].numel()))
+        st = self._flow_state(packed_init_noises, ql, packed_vae_token_indexes, packed_text_indexes,
+                              packed_vae_position_ids, packed_text_ids, 1)
+        st["v_all"] = torch.empty((big["n"], self.patch_latent_dim), dtype=BF16, device=dev)
+        st["t_emb"] = self.time_embedder(ts.to(dev))
+        for key, lay in lays.items():
+            st[key] = self._build_flow_batch_plan(lay, branches)
+        rows = big["rows"]
+        i32 = lambda t: torch.as_tensor(t).to(dev, torch.int32).contiguous()
+        none = torch.full_like(rows[0], -1)
+        st["seg"] = i32(big["seg"])
+        st["row_main"] = i32(rows[0])
+        st["row_text"] = i32(rows[1] if rows.shape[0] > 1 else none)
+        st["row_img"] = i32(rows[2] if rows.shape[0] > 2 else none)
+        st["sT"] = torch.tensor([float(x) for x in cfg_text_scale], dtype=torch.float32, device=dev)
+        st["sI"] = torch.tensor([float(x) for x in cfg_img_scale], dtype=torch.float32, device=dev)
+        st["renorm_min"] = torch.tensor([float(x) for x in cfg_renorm_min], dtype=torch.float32, device=dev)
+        st["renorm_type"] = i32([ops.RENORM[x] for x in cfg_renorm_type])
+        st["cfg_ws"] = ops.cfg_batch_workspace(st["M"], R, dev)
+        cfg_tab = i32([[int(x) for x in row] for row in cfg_on]).reshape(len(cfg_on), R)
+        runner = BatchFlowRunner(self, st, dts.tolist(), full, cfg_tab, ql, big["n"])
+        for i in range(runner.num_steps):
+            runner.step(i)
+        return list(runner.latents())
 
     # ------------------------------------------------------------------------------------------
     # text decode
@@ -1020,7 +1278,7 @@ class FlowRunner:
     captured ONCE per branch set as a CUDA graph and replayed for the remaining steps."""
 
     def __init__(self, model: Bagel, st, dts, cfg_on, scales, renorm_min, renorm_type, nbmax, seqlens,
-                 enable_taylorseer: bool = False):
+                 enable_taylorseer: bool = False, rows_max: Optional[int] = None):
         self.model, self.st, self.dts, self.cfg_on = model, st, dts, cfg_on
         self.scales, self.renorm_min, self.renorm_type, self.nbmax = scales, renorm_min, renorm_type, nbmax
         self.seqlens = seqlens
@@ -1036,7 +1294,8 @@ class FlowRunner:
         lcfg = model.language_model.model.config
         Hd, Id = lcfg.hidden_size, lcfg.intermediate_size
         qkv_o = (lcfg.num_attention_heads * 2 + lcfg.num_key_value_heads * 2) * lcfg.head_dim
-        flops_step = 2.0 * nbmax * st["n"] * lcfg.num_hidden_layers * Hd * (qkv_o + 3 * Id)
+        rows = nbmax * st["n"] if rows_max is None else rows_max      # packed rows of the largest LM call of a step
+        flops_step = 2.0 * rows * lcfg.num_hidden_layers * Hd * (qkv_o + 3 * Id)
         self.use_cuda_graph = bool(getattr(model, "use_cuda_graph", True)) and flops_step / 1.0e15 < 0.05
         self._graphs: Dict[str, Any] = {}
         self._graph_gen: Dict[str, int] = {}
@@ -1119,3 +1378,26 @@ class FlowRunner:
 
     def latents(self):
         return self.st["x"].split((self.seqlens - 2).tolist())
+
+
+class BatchFlowRunner(FlowRunner):
+    """FlowRunner of Bagel.generate_image_batch: the same launch / capture / workspace-generation logic, with the
+    batch's velocity evaluation and bagel_cfg_euler_step_batch as the step body. Besides t_cur and dt_cur, the step
+    copies its row of the device CFG table [steps, R] into cfg_cur, so one captured graph per plan serves every step."""
+
+    def __init__(self, model: Bagel, st, dts, full, cfg_tab: torch.Tensor, seqlens, rows_max: int):
+        super().__init__(model, st, dts, full, None, None, None, 2 if "full" in st else 1, seqlens, rows_max=rows_max)
+        self.cfg_tab = cfg_tab
+        self.cfg_cur = torch.zeros_like(cfg_tab[0])
+
+    @torch.no_grad()
+    def step(self, i: int):
+        self.cfg_cur.copy_(self.cfg_tab[i])
+        super().step(i)
+
+    def _body(self, key: str):
+        m, st = self.model, self.st
+        m._velocity_batch(st, key, self.t_cur, st["x"])
+        ops.cfg_euler_step_batch(st["v_all"], st["seg"], st["row_main"], st["row_text"], st["row_img"], st["x"],
+                                 st["cfg_ws"], st["sT"], st["sI"], st["renorm_min"], st["renorm_type"], self.cfg_cur,
+                                 self.dt_cur)

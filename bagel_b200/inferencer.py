@@ -12,7 +12,7 @@ those are absent.
 from __future__ import annotations
 
 from copy import deepcopy
-from typing import Any, Dict, List, Optional, Union
+from typing import Any, Dict, List, Optional, Sequence, Union
 
 import torch
 
@@ -173,6 +173,93 @@ class InterleaveInferencer:
             timestep_shift=timestep_shift, num_timesteps=num_timesteps, cfg_renorm_min=cfg_renorm_min,
             cfg_renorm_type=cfg_renorm_type, enable_taylorseer=enable_taylorseer))
         return outputs
+
+    # per-request defaults of gen_image_batch: those of interleave_inference
+    GEN_BATCH_DEFAULTS = dict(cfg_text_scale=3.0, cfg_img_scale=1.5, cfg_interval=(0.4, 1.0), cfg_renorm_min=0.0,
+                              cfg_renorm_type="global", image_shapes=(1024, 1024))
+
+    @torch.no_grad()
+    def gen_image_batch(self, requests: Sequence[Dict[str, Any]], num_timesteps: int = 50,
+                        timestep_shift: float = 3.0) -> List[Any]:
+        """Text-to-image and edit requests in one packed denoising run; returns one PIL image per request.
+
+        Each request is a dict: `text` (required), `image` (optional PIL image: an edit, whose output takes the resized
+        input's shape), `image_shapes` (T2I only), `cfg_text_scale`, `cfg_img_scale`, `cfg_interval`, `cfg_renorm_min`,
+        `cfg_renorm_type` (defaults of interleave_inference) and `seed`. Request i with seed s gets what
+        `torch.manual_seed(s); inferencer(image=..., text=..., **its settings)` gives it alone (think=False): its VAE-encode
+        noise comes from the CUDA generator seeded with s in its own latent shape, its init noise from a CPU generator
+        seeded with s. `seed=None` draws one from torch.default_generator.
+
+        The contexts are those interleave_inference builds per request (T2I: main [text], cfg_text empty, cfg_img
+        [text]; edit: main [VAE + ViT image, text], cfg_text [VAE + ViT image], cfg_img [text]), built for all requests
+        at once: one VAE image round (each image encoded on its own, so that its latents do not depend on the padding
+        a batch would add), one SigLIP call and one ViT round, one text prefill for the main contexts and one for the
+        cfg_img contexts; cfg_text is a copy of the main caches after the image rounds. One Bagel.generate_image_batch
+        denoises every request; the VAE decodes each image on its own."""
+        from .transforms import pil_img2rgb
+        m = self.model
+        R = len(requests)
+        if R == 0:
+            return []
+        unknown = [k for r in requests for k in r if k not in ("text", "image", "seed", *self.GEN_BATCH_DEFAULTS)]
+        if unknown:
+            raise ValueError(f"gen_image_batch: unknown request keys {sorted(set(unknown))}")
+        reqs = [{**self.GEN_BATCH_DEFAULTS, **r} for r in requests]
+        seeds = [int(r["seed"]) if r.get("seed") is not None else int(torch.randint(0, 2 ** 32, (1,), dtype=torch.int64))
+                 for r in reqs]
+        images = [None if r.get("image") is None else self.vae_transform.resize_transform(pil_img2rgb(r["image"]))
+                  for r in reqs]
+        shapes = [tuple(im.size[::-1]) if im is not None else tuple(r["image_shapes"]) for im, r in zip(images, reqs)]
+        L = m.config.llm_config.num_hidden_layers
+        kv, rope = [0] * R, [0] * R
+        cache = NaiveCache(L)
+        if any(im is not None for im in images):
+            if self.vae_model is None:
+                raise NotImplementedError("edit requests need the VAE encoder")
+            gi, kv, rope, tensors = m.prepare_vae_image_round(kv, rope, images, self.vae_transform, self.new_token_ids,
+                                                              return_tensors=True)
+            gi.pop("padded_images")
+            lat_shapes = gi.pop("patchified_vae_latent_shapes")
+            present = [q for q in range(R) if images[q] is not None]
+            latents = [self._encode_image(t, seeds[q]) for t, q in zip(tensors, present)]
+            cache = m._prefill_vae_latents(cache, m._patchify_latents(latents, lat_shapes), **gi)
+            gi, kv, rope = m.prepare_vit_image_round(kv, rope, images, self.vit_transform, self.new_token_ids)
+            cache = m.forward_cache_update_vit(cache, **gi)
+        text_ctx = (deepcopy(cache), kv, rope)       # text-dropped branch = everything before the text
+        texts = [r["text"] for r in reqs]
+        gi, kv, rope = m.prepare_prompts(kv, rope, texts, self.tokenizer, self.new_token_ids)
+        cache = m.forward_cache_update_text(cache, **gi)
+        gi, kv_i, rope_i = m.prepare_prompts([0] * R, [0] * R, texts, self.tokenizer, self.new_token_ids)
+        cache_img = m.forward_cache_update_text(NaiveCache(L), **gi)
+        gi = m.prepare_vae_latent(kv, rope, shapes, self.new_token_ids,
+                                  generators=[torch.Generator().manual_seed(s) for s in seeds])
+        ct = m.prepare_vae_latent_cfg(text_ctx[1], text_ctx[2], shapes)
+        ci = m.prepare_vae_latent_cfg(kv_i, rope_i, shapes)
+        latents = m.generate_image_batch(
+            past_key_values=cache, cfg_text_past_key_values=text_ctx[0], cfg_img_past_key_values=cache_img,
+            num_timesteps=num_timesteps, timestep_shift=timestep_shift,
+            **{k: [r[k] for r in reqs] for k in ("cfg_text_scale", "cfg_img_scale", "cfg_interval", "cfg_renorm_min",
+                                                 "cfg_renorm_type")},
+            **gi,
+            cfg_text_packed_position_ids=ct["cfg_packed_position_ids"],
+            cfg_text_packed_query_indexes=ct["cfg_packed_query_indexes"],
+            cfg_text_key_values_lens=ct["cfg_key_values_lens"],
+            cfg_text_packed_key_value_indexes=ct["cfg_packed_key_value_indexes"],
+            cfg_img_packed_position_ids=ci["cfg_packed_position_ids"],
+            cfg_img_packed_query_indexes=ci["cfg_packed_query_indexes"],
+            cfg_img_key_values_lens=ci["cfg_key_values_lens"],
+            cfg_img_packed_key_value_indexes=ci["cfg_packed_key_value_indexes"])
+        return [self.decode_image(lat, hw) for lat, hw in zip(latents, shapes)]
+
+    def _encode_image(self, image: torch.Tensor, seed: int) -> torch.Tensor:
+        """VAE-encode one transformed image [C, H, W] on its own, with its DiagonalGaussian noise drawn as a single
+        request seeded with `seed` draws it: from the default CUDA generator of the VAE's device, seeded with `seed`,
+        in the image's own latent shape. The caller's CUDA RNG state is restored. Returns its latent [z, h, w]."""
+        dev = torch.device(getattr(self.vae_model, "device", self.model.device))
+        with torch.random.fork_rng(devices=[dev]):
+            with torch.cuda.device(dev):
+                torch.cuda.manual_seed(seed)
+            return self.vae_model.encode(image[None].to(torch.float32))[0]    # the fp32 canvas prepare_vae_images builds
 
     def __call__(self, image=None, text: Optional[str] = None, **kargs) -> Dict[str, Any]:
         result = {"image": None, "text": None}

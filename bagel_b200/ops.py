@@ -328,6 +328,39 @@ def cfg_euler_step(v, v_text, v_img, rows, x, norms_ws, cfg_text_scale, cfg_img_
     _cabi.check(rc, "bagel_cfg_euler_step")
 
 
+def cfg_batch_workspace(M: int, R: int, device) -> torch.Tensor:
+    """fp32 workspace of cfg_euler_step_batch for M latent rows of R requests."""
+    return torch.zeros(2 * M + 2 * R, dtype=torch.float32, device=device)
+
+
+def cfg_euler_step_batch(v, seg, row_main, row_text, row_img, x, workspace, cfg_text_scale, cfg_img_scale, renorm_min,
+                         renorm_type, cfg_on, dt_dev):
+    """Per-request CFG + renorm + Euler step (see include/bagel_b200.h): latent row r of request seg[r] reads rows
+    row_main[r] / row_text[r] / row_img[r] (-1: no such branch) of v; a request's rows are contiguous in seg.
+    Per-request parameters are device arrays of length R: scales / renorm_min fp32, renorm_type (ops.RENORM values) and
+    cfg_on int32; dt_dev fp32[1]; workspace from cfg_batch_workspace."""
+    _req(x, torch.float32, "x")
+    M, Cc = x.shape
+    assert x.is_contiguous()
+    _req(v, torch.bfloat16, "v")
+    for t, nm in ((seg, "seg"), (row_main, "row_main"), (row_text, "row_text"), (row_img, "row_img")):
+        _req(t, torch.int32, nm)
+        assert t.numel() >= M, f"{nm}: one entry per latent row"
+    R = cfg_on.numel()
+    for t, dt, nm in ((cfg_text_scale, torch.float32, "cfg_text_scale"), (cfg_img_scale, torch.float32, "cfg_img_scale"),
+                      (renorm_min, torch.float32, "renorm_min"), (renorm_type, torch.int32, "renorm_type"),
+                      (cfg_on, torch.int32, "cfg_on")):
+        _req(t, dt, nm)
+        assert t.numel() == R, f"{nm}: one entry per request"
+    _req(dt_dev, torch.float32, "dt_dev"); _req(workspace, torch.float32, "workspace")
+    assert workspace.numel() >= 2 * M + 2 * R and v.shape[-1] >= Cc
+    rc = _cabi.lib().bagel_cfg_euler_step_batch(_ptr(v), v.stride(0), _ptr(seg), _ptr(row_main), _ptr(row_text),
+                                                _ptr(row_img), _ptr(x), M, Cc, R, _ptr(cfg_text_scale),
+                                                _ptr(cfg_img_scale), _ptr(renorm_min), _ptr(renorm_type), _ptr(cfg_on),
+                                                _ptr(dt_dev), _ptr(workspace), _stream())
+    _cabi.check(rc, "bagel_cfg_euler_step_batch")
+
+
 def cast_f32_to_bf16(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     _req(x, torch.float32, "x")
     assert x.is_contiguous()

@@ -279,16 +279,21 @@ class Qwen2Model:
         v = torch.empty((L, plan.total_kv, w), dtype=BF16, device=self.device)
         return k, v
 
-    def place_context(self, cache: NaiveCache, rows: torch.Tensor, kbuf, vbuf):
+    def place_context(self, cache: NaiveCache, rows: torch.Tensor, kbuf, vbuf, src_rows: Optional[torch.Tensor] = None):
         """Copy every layer's cached K/V rows to `rows` (int32, on the device) of the merged buffers (reference
-        :565-569)."""
+        :565-569). src_rows (int32, on the device, as many as `rows`): place only these cache rows, cache row
+        src_rows[i] to rows[i] (the requests of a batch that take part in one CFG branch)."""
         cfg = self.config
         m, w = rows.numel(), cfg.num_key_value_heads * cfg.head_dim
         for li in range(cfg.num_hidden_layers):
             pk, pv = cache.key_cache[li], cache.value_cache[li]
-            assert pk is not None and pk.shape[0] == m, "cache rows must match key_values_lens"
-            ops.copy_rows(pk.reshape(m, w), kbuf[li], dst_rows=rows, M=m)
-            ops.copy_rows(pv.reshape(m, w), vbuf[li], dst_rows=rows, M=m)
+            if src_rows is None:
+                assert pk is not None and pk.shape[0] == m, "cache rows must match key_values_lens"
+            else:
+                assert pk is not None and src_rows.numel() == m, "one cache row per destination row"
+            n = pk.shape[0]
+            ops.copy_rows(pk.reshape(n, w), kbuf[li], src_rows=src_rows, dst_rows=rows, M=m)
+            ops.copy_rows(pv.reshape(n, w), vbuf[li], src_rows=src_rows, dst_rows=rows, M=m)
 
     # ----------------------------------------------------------------------------------------------
     def run_layers(self, x: torch.Tensor, plan: ForwardPlan, kbuf: torch.Tensor, vbuf: torch.Tensor,

@@ -178,6 +178,24 @@ int bagel_cfg_euler_step(const void* v, const void* v_text, const void* v_img, l
                          float* x, float* norms_ws, int M, int C, float cfg_text_scale, float cfg_img_scale,
                          float renorm_min, int renorm_type, float dt, const float* dt_dev, void* stream);
 
+/* bagel_cfg_euler_step for a batch of independent requests (Bagel.generate_image_batch), x fp32 [M, C] in place.
+ *   Latent row r belongs to request seg[r] in [0, R); the rows of one request are contiguous (one run of seg). Row r
+ *   reads rows row_main[r], row_text[r], row_img[r] of the bf16 llm2vae output v (row pitch ldv); row_text / row_img
+ *   are -1 when the request has no such branch.
+ *   Per request q (device arrays of length R): cfg_text_scale[q], cfg_img_scale[q], renorm_min[q], renorm_type[q]
+ *   (0 "global", 1 "channel", 2 "text_channel"; mixed in one launch) and cfg_on[q] for this step. Row r takes text CFG
+ *   when cfg_on[q] != 0, row_text[r] >= 0 and cfg_text_scale[q] > 1, and image CFG inside it when also row_img[r] >= 0
+ *   and cfg_img_scale[q] > 1; otherwise x -= bf16(v * dt). Every rounding point is that of bagel_cfg_euler_step with
+ *   the request's parameters. "global" norms are summed over the request's own rows only, per row and then in a fixed
+ *   order (no atomics): two launches give the same bits. The work per step is O(M + R).
+ *   dt_dev: device pointer to the step size (required). workspace: 4-byte words [2 * M + 2 * R] of device memory
+ *   (contents need no initialisation).
+ *   No host reads, no allocations: capturable once for every step of a run. C <= 128. */
+int bagel_cfg_euler_step_batch(const void* v, long long ldv, const int* seg, const int* row_main, const int* row_text,
+                               const int* row_img, float* x, int M, int C, int R, const float* cfg_text_scale,
+                               const float* cfg_img_scale, const float* renorm_min, const int* renorm_type,
+                               const int* cfg_on, const float* dt_dev, float* workspace, void* stream);
+
 /* y[i] = bf16(x[i]) — the autocast cast in front of vae2llm (modeling/bagel/bagel.py:803). */
 int bagel_cast_f32_to_bf16(const float* x, void* y, long long n, void* stream);
 
