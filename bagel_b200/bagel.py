@@ -15,9 +15,11 @@ What is different underneath (GPU-first, not a port):
 """
 from __future__ import annotations
 
+import numbers
 import warnings
-from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 
+import numpy as np
 import torch
 
 from . import ops
@@ -296,8 +298,15 @@ class Bagel:
     # packers
     # ------------------------------------------------------------------------------------------
     def prepare_prompts(self, curr_kvlens, curr_rope, prompts, tokenizer, new_token_ids):
+        return self.prepare_prompts_round(curr_kvlens, curr_rope, list(prompts), tokenizer, new_token_ids)
+
+    def prepare_prompts_round(self, curr_kvlens, curr_rope, prompts, tokenizer, new_token_ids):
+        """One text round of a batch of independent requests, with prepare_vit_image_round's contract: prompts[i] is
+        request i's text or None. A request with a text gets the layout prepare_prompts gives that text alone
+        ([bos] + tokens + [eos]); a request without one contributes zero query tokens, its cached rows are carried
+        unchanged and its kv len and rope position stay."""
         bos, eos = new_token_ids["bos_token_id"], new_token_ids["eos_token_id"]
-        ids = [[bos] + list(tokenizer.encode(p)) + [eos] for p in prompts]
+        ids = [[] if p is None else [bos] + list(tokenizer.encode(p)) + [eos] for p in prompts]
         tl = torch.tensor([len(x) for x in ids], dtype=torch.int64)
         cl = torch.tensor(list(curr_kvlens), dtype=torch.int64)
         rope = torch.tensor(list(curr_rope), dtype=torch.int64)
@@ -964,9 +973,11 @@ class Bagel:
 
     @torch.no_grad()
     def generate_text_batch(self, past_key_values: NaiveCache, packed_key_value_indexes, key_values_lens,
-                            packed_start_tokens, packed_query_position_ids, max_length: int, do_sample: bool = False,
-                            temperature: float = 1.0, end_token_id: Optional[int] = None,
-                            seeds: Optional[Sequence[int]] = None) -> List[torch.Tensor]:
+                            packed_start_tokens, packed_query_position_ids, max_length: Union[int, Sequence[int]],
+                            do_sample: Union[bool, Sequence[bool]] = False,
+                            temperature: Union[float, Sequence[float]] = 1.0, end_token_id: Optional[int] = None,
+                            seeds: Optional[Sequence[int]] = None,
+                            keys: Optional[Sequence[int]] = None) -> List[torch.Tensor]:
         """Decode a batch of independent requests (same inputs as generate_text). Returns one LongTensor per request on
         the model's device: its tokens from the start token up to, not including, its own `end_token_id`, at most
         `max_length` of them. A finished request's token, sequence length and position freeze while the others go on.
@@ -974,44 +985,78 @@ class Bagel:
         Greedy picks the first maximum (argmax_rows); do_sample=True draws from softmax(logits / temperature) on the
         device (Gumbel-max over Philox4x32-10, ops.sample_rows). Request i's draws are keyed by (seed, i): `seeds=None`
         takes one 32-bit base seed from torch.default_generator (so torch.manual_seed fixes it) for every request,
-        otherwise request i uses seeds[i]. Either way a step is one CUDA-graph replay (after an eager first step), and
-        the host only reads the device's count of unfinished requests, lagged, to stop early."""
+        otherwise request i uses seeds[i]. `keys` (one 64-bit Philox key per request) replaces that key, for a caller
+        whose draws must not depend on a request's index. Either way a step is one CUDA-graph replay (after an eager
+        first step), and the host only reads the device's count of unfinished requests, lagged, to stop early.
+
+        max_length, do_sample and temperature may each be one value per request instead of one for all. The step then
+        picks every row with ops.sample_rows_mixed (greedy rows take argmax_rows' pick, sampled rows sample_rows' pick
+        at their own temperature) and stops each request at its own limit with ops.decode_advance_stop_limits."""
         if self.dtype_mode == "B":
             raise NotImplementedError("generate_text_batch: the device-resident decode loop is implemented for dtype_mode='A'")
-        if do_sample and not (0.0 < float(temperature) < float("inf")):
-            raise ValueError("generate_text_batch: do_sample=True needs a finite temperature > 0")
         dev = self.device
         B = int(torch.as_tensor(key_values_lens).numel())
-        if max_length <= 0:
+        per_request = not all(isinstance(x, numbers.Real) for x in (max_length, do_sample, temperature))
+        if per_request:
+            max_length, do_sample, temperature = (
+                [x] * B if isinstance(x, numbers.Real) else list(x) for x in (max_length, do_sample, temperature))
+            for name, x in (("max_length", max_length), ("do_sample", do_sample), ("temperature", temperature)):
+                if len(x) != B:
+                    raise ValueError(f"generate_text_batch: {name} has {len(x)} entries for {B} requests")
+            if any(s and not (0.0 < float(t) < float("inf")) for s, t in zip(do_sample, temperature)):
+                raise ValueError("generate_text_batch: do_sample=True needs a finite temperature > 0")
+            limits = [max(int(n), 0) for n in max_length]
+            steps_max = max(limits, default=0)
+        else:
+            if do_sample and not (0.0 < float(temperature) < float("inf")):
+                raise ValueError("generate_text_batch: do_sample=True needs a finite temperature > 0")
+            steps_max = max_length
+        if steps_max <= 0:
             return [torch.zeros(0, dtype=torch.int64, device=dev) for _ in range(B)]
-        if seeds is None:
-            base = int(torch.randint(0, 2 ** 32, (1,), dtype=torch.int64))
-            seeds = [base] * B
-        elif len(seeds) != B:
-            raise ValueError(f"generate_text_batch: {len(seeds)} seeds for {B} requests")
+        if keys is None:
+            if seeds is None:
+                base = int(torch.randint(0, 2 ** 32, (1,), dtype=torch.int64))
+                seeds = [base] * B
+            elif len(seeds) != B:
+                raise ValueError(f"generate_text_batch: {len(seeds)} seeds for {B} requests")
+            keys = [(int(sd) & 0xFFFFFFFF) | (i << 32) for i, sd in enumerate(seeds)]
+        elif len(keys) != B:
+            raise ValueError(f"generate_text_batch: {len(keys)} keys for {B} requests")
         d = self._decode_state(past_key_values, key_values_lens, packed_start_tokens, packed_query_position_ids,
-                               max_length)
+                               steps_max)
         body, logits, history, step_dev = d["body"], d["logits"], d["history"], d["step_dev"]
-        keys = torch.tensor([(int(sd) & 0xFFFFFFFF) | (i << 32) for i, sd in enumerate(seeds)], dtype=torch.int64,
-                            device=dev)
+        keys = torch.from_numpy(np.array([int(k) & 0xFFFFFFFFFFFFFFFF for k in keys], dtype=np.uint64).view(np.int64)).to(dev)
         nxt = torch.empty(B, dtype=torch.int64, device=dev)
         finished = torch.zeros(B, dtype=torch.int32, device=dev)
         unfinished = torch.full((1,), B, dtype=torch.int32, device=dev)
 
-        def step_fn():
-            body()
-            if do_sample:
-                ops.sample_rows(logits, temperature, keys, step_dev, nxt)
-            else:
-                ops.argmax_rows(logits, nxt)
-            ops.decode_advance_stop(d["seq_len"], d["pos"], d["tokens"], d["tokens32"], nxt, history, step_dev, finished,
-                                    unfinished, end_token_id, self.HISTORY_PAD)
+        if per_request:
+            # 1.0f / T in fp32, as bagel_sample_rows_bf16 derives its inverse temperature; 0 marks a greedy row. A request
+            # with no budget runs one step (the kernel's smallest) and is cut to nothing below.
+            inv_t = torch.from_numpy(np.array([np.float32(1.0) / np.float32(t) if s else np.float32(0.0)
+                                               for s, t in zip(do_sample, temperature)], dtype=np.float32)).to(dev)
+            lim_dev = torch.tensor([max(n, 1) for n in limits], dtype=torch.int32, device=dev)
+
+            def step_fn():
+                body()
+                ops.sample_rows_mixed(logits, inv_t, keys, step_dev, nxt)
+                ops.decode_advance_stop_limits(d["seq_len"], d["pos"], d["tokens"], d["tokens32"], nxt, history,
+                                               step_dev, finished, unfinished, end_token_id, lim_dev, self.HISTORY_PAD)
+        else:
+            def step_fn():
+                body()
+                if do_sample:
+                    ops.sample_rows(logits, temperature, keys, step_dev, nxt)
+                else:
+                    ops.argmax_rows(logits, nxt)
+                ops.decode_advance_stop(d["seq_len"], d["pos"], d["tokens"], d["tokens32"], nxt, history, step_dev,
+                                        finished, unfinished, end_token_id, self.HISTORY_PAD)
 
         count_host = torch.zeros(2, dtype=torch.int32, pin_memory=True)
         pending = None        # (event, slot) of the last count copy not yet read
         graph = None
         steps = 0
-        for step in range(max_length):
+        for step in range(steps_max):
             if graph is not None:
                 graph.replay()
             elif step == 1 and self.use_cuda_graph:
@@ -1034,6 +1079,8 @@ class Bagel:
                 pending = (ev, slot)
         hist = history[:steps]
         lens = (hist != self.HISTORY_PAD).sum(0).tolist()
+        if per_request:
+            lens = [min(n, lim) for n, lim in zip(lens, limits)]
         return [hist[:n, i].clone() for i, n in enumerate(lens)]
 
     @torch.no_grad()

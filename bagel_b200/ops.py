@@ -508,6 +508,41 @@ def decode_advance_stop(seq_len, pos, tokens, tokens32, next_tokens, history, st
     _cabi.check(rc, "bagel_decode_advance_stop")
 
 
+def sample_rows_mixed(logits: torch.Tensor, inv_temperature: torch.Tensor, keys: torch.Tensor, step_dev: torch.Tensor,
+                      tokens: torch.Tensor, tokens32: Optional[torch.Tensor] = None):
+    """Per-row sample_rows / argmax_rows: row b is greedy where inv_temperature[b] == 0, else a draw at
+    1 / T = inv_temperature[b] (fp32, on the device); see include/bagel_b200.h."""
+    _req(logits, torch.bfloat16, "logits"); _req(inv_temperature, torch.float32, "inv_temperature")
+    _req(keys, torch.int64, "keys"); _req(step_dev, torch.int32, "step_dev"); _req(tokens, torch.int64, "tokens")
+    _opt(tokens32, torch.int32, "tokens32")
+    B, V = logits.shape
+    assert inv_temperature.numel() == keys.numel() == tokens.numel() == B and (tokens32 is None or tokens32.numel() == B)
+    rc = _cabi.lib().bagel_sample_rows_mixed_bf16(_ptr(logits), logits.stride(0), B, V, _ptr(inv_temperature),
+                                                  _ptr(keys), _ptr(step_dev), _ptr(tokens), _ptr(tokens32), _stream())
+    _cabi.check(rc, "bagel_sample_rows_mixed_bf16")
+
+
+def decode_advance_stop_limits(seq_len, pos, tokens, tokens32, next_tokens, history, step_dev, finished, unfinished,
+                               end_token_id: Optional[int], max_length: torch.Tensor, pad: int):
+    """decode_advance_stop with a limit per request (max_length int32 [B] on the device; history [rows, B]); see
+    include/bagel_b200.h."""
+    for t, dt, nm in ((seq_len, torch.int32, "seq_len"), (pos, torch.int64, "pos"), (tokens, torch.int64, "tokens"),
+                      (tokens32, torch.int32, "tokens32"), (next_tokens, torch.int64, "next_tokens"),
+                      (history, torch.int64, "history"), (step_dev, torch.int32, "step_dev"),
+                      (finished, torch.int32, "finished"), (unfinished, torch.int32, "unfinished"),
+                      (max_length, torch.int32, "max_length")):
+        _req(t, dt, nm)
+    B = seq_len.numel()
+    assert pos.numel() == tokens.numel() == tokens32.numel() == next_tokens.numel() == finished.numel() == B
+    assert max_length.numel() == B
+    assert history.dim() == 2 and history.is_contiguous() and history.shape[1] == B
+    rc = _cabi.lib().bagel_decode_advance_stop_limits(
+        _ptr(seq_len), _ptr(pos), _ptr(tokens), _ptr(tokens32), _ptr(next_tokens), _ptr(history), _ptr(step_dev),
+        _ptr(finished), _ptr(unfinished), -1 if end_token_id is None else int(end_token_id), _ptr(max_length),
+        history.shape[0], int(pad), B, _stream())
+    _cabi.check(rc, "bagel_decode_advance_stop_limits")
+
+
 def taylor_update(feature: torch.Tensor, factors: torch.Tensor, n_deriv: int, dist: int, rows: Optional[int] = None):
     """TaylorSeer derivative_approximation (cache_utils/taylorseer.py:12-32) on factor planes [orders, cap_rows, H]
     (in place): plane 0 <- feature, plane i+1 <- bf16(bf16(plane_i_new - plane_i_old) / dist) for i < n_deriv."""

@@ -58,6 +58,31 @@ class NaiveCache:
         return 0 if self.key_cache[0] is None else self.key_cache[0].shape[0]
 
 
+def gather_requests(cache: NaiveCache, key_values_lens, members) -> NaiveCache:
+    """A new packed cache holding only the blocks of requests `members` (in that order) of `cache`, whose request q
+    owns key_values_lens[q] rows in request order: one copy_rows per layer and K / V. When the members' blocks are
+    already the whole cache, the new cache shares its tensors (cache tensors are replaced, never written in place)."""
+    kv = torch.as_tensor(key_values_lens).to("cpu", torch.int64)
+    start = torch.cumsum(kv, 0) - kv
+    m = torch.as_tensor(list(members), dtype=torch.int64)
+    src = _ranges(start[m], kv[m])
+    out = NaiveCache(cache.num_layers)
+    n = cache.seq_lens
+    if src.numel() == 0:
+        return out
+    if src.numel() == n and torch.equal(src, torch.arange(n)):
+        out.key_cache, out.value_cache = dict(cache.key_cache), dict(cache.value_cache)
+        return out
+    rows = src.to(cache.key_cache[0].device, torch.int32)
+    for li in range(cache.num_layers):
+        for srcs, dsts in ((cache.key_cache, out.key_cache), (cache.value_cache, out.value_cache)):
+            t = srcs[li]
+            dst = torch.empty((rows.numel(), *t.shape[1:]), dtype=t.dtype, device=t.device)
+            ops.copy_rows(t.reshape(n, -1), dst.reshape(rows.numel(), -1), src_rows=rows)
+            dsts[li] = dst
+    return out
+
+
 @dataclass
 class BaseNavitOutputWithPast:
     packed_query_sequence: torch.Tensor = None

@@ -259,6 +259,24 @@ int bagel_decode_advance_stop(int* seq_len, long long* pos, long long* tokens, i
                               long long* history, int* step_dev, int* finished, int* unfinished, long long end_token_id,
                               int max_length, long long pad, int B, void* stream);
 
+/* Per-request decode settings (Bagel.generate_text_batch with per-request max_length / do_sample / temperature), one
+ * launch each, graph-replayable:
+ *   bagel_sample_rows_mixed_bf16: row b with inv_temperature[b] == 0 takes bagel_argmax_rows_bf16's pick (first maximum,
+ *     same NaN / -inf handling); any other row takes exactly bagel_sample_rows_bf16's pick at 1 / T = inv_temperature[b]
+ *     (the caller stores 1.0f / temperature, rounded as bagel_sample_rows_bf16 computes it). keys and step_dev are as in
+ *     bagel_sample_rows_bf16 and are read by sampled rows only; tokens32 may be NULL.
+ *   bagel_decode_advance_stop_limits: bagel_decode_advance_stop with a limit per request: request b finishes when
+ *     next[b] == end_token_id or step + 1 >= max_length[b]. history is [history_rows, B]; rows at step >= history_rows
+ *     are not written. With every max_length[b] == history_rows it computes what bagel_decode_advance_stop computes with
+ *     max_length = history_rows. B <= 1024. */
+int bagel_sample_rows_mixed_bf16(const void* logits, long long ld, int B, int V, const float* inv_temperature,
+                                 const long long* keys, const int* step_dev, long long* tokens, int* tokens32,
+                                 void* stream);
+int bagel_decode_advance_stop_limits(int* seq_len, long long* pos, long long* tokens, int* tokens32,
+                                     const long long* next, long long* history, int* step_dev, int* finished,
+                                     int* unfinished, long long end_token_id, const int* max_length, int history_rows,
+                                     long long pad, int B, void* stream);
+
 /* TaylorSeer step cache (reference modeling/cache_utils/taylorseer.py, enabled by generate_image(enable_taylorseer=True),
  * modeling/bagel/bagel.py:678-684; decoder-layer hooks modeling/bagel/qwen2_navit.py:773-777, 824-829).
  * factors: bf16 planes [order][rows][H], plane_stride elements apart, of the last decoder layer's output.

@@ -55,6 +55,15 @@ for (lk, Hq, Hk) in (([300, 17, 0, 1100], 28, 4), ([33, 64], 8, 8), ([90], 4, 2)
     od = ops.attn_varlen(q, k, v, cq, ck, 1, max(lk), True, seqused_k=torch.tensor(lk, dtype=torch.int32, device=dev))
 lg = torch.randn(3, 1000, device=dev, generator=g).to(bf); tk = torch.empty(3, dtype=torch.int64, device=dev)
 ops.argmax_rows(lg, tk, torch.empty(3, dtype=torch.int32, device=dev))
+# per-request decode settings: mixed greedy / sampled rows (unaligned ld), per-row stop limits
+lg2 = torch.randn(4, 1031, device=dev, generator=g).to(bf)[:, :1029]; tk2 = torch.empty(4, dtype=torch.int64, device=dev)
+sd = torch.zeros(1, dtype=torch.int32, device=dev)
+ops.sample_rows_mixed(lg2, torch.tensor([0.0, 2.0, 0.0, 1.0], device=dev), torch.arange(4, device=dev), sd, tk2,
+                      torch.empty(4, dtype=torch.int32, device=dev))
+i32 = lambda *v: torch.tensor(v, dtype=torch.int32, device=dev)
+ops.decode_advance_stop_limits(i32(3, 4, 5, 6), torch.arange(4, device=dev), tk2.clone(), tk2.to(torch.int32), tk2,
+                               torch.zeros(3, 4, dtype=torch.int64, device=dev), sd, i32(0, 0, 1, 0), i32(4), 5,
+                               i32(1, 3, 2, 5), -1)
 fac = torch.zeros(7, 40, 256, device=dev, dtype=bf); ft = torch.randn(37, 256, device=dev, generator=g).to(bf)
 ops.taylor_update(ft, fac[:, 2:39], 0, 1); ops.taylor_update(ft, fac[:, 2:39], 1, 3); ops.taylor_eval(fac[:, 2:39], 2, 2, ft)
 torch.cuda.synchronize()
