@@ -176,6 +176,41 @@ def _flow_batch_schedule(num_timesteps: int, timestep_shift: float, cfg_interval
     return ts, dts, cfg_on, full
 
 
+def _sampling_filters(B: int, do_sample, top_k, top_p, min_p,
+                      who: str = "generate_text_batch") -> Optional[Tuple[List[int], List[float], List[float]]]:
+    """generate_text_batch's top_k / top_p / min_p (each None, one value, or one per request), checked: per-request
+    lists (0, 1.0, 0.0 where off) for ops.sample_rows_filtered, or None when no sampled request sets a filter."""
+    def expand(name, x):
+        if x is None or isinstance(x, numbers.Real):
+            return [x] * B
+        x = list(x)
+        if len(x) != B:
+            raise ValueError(f"{who}: {name} has {len(x)} entries for {B} requests")
+        return x
+
+    def top_k_ok(k):
+        return isinstance(k, numbers.Integral) and not isinstance(k, bool) and k >= 0
+
+    def real(v):
+        return isinstance(v, numbers.Real) and not isinstance(v, bool)
+
+    ks = [0 if k is None else k for k in expand("top_k", top_k)]
+    ps = [1.0 if p is None else p for p in expand("top_p", top_p)]
+    ms = [0.0 if m is None else m for m in expand("min_p", min_p)]
+    if not all(top_k_ok(k) for k in ks):
+        raise ValueError(f"{who}: top_k must be None or an int >= 0, got {top_k!r}")
+    if not all(real(p) and 0.0 < p <= 1.0 for p in ps):
+        raise ValueError(f"{who}: top_p must be None or in (0, 1], got {top_p!r}")
+    if not all(real(m) and 0.0 <= m < 1.0 for m in ms):
+        raise ValueError(f"{who}: min_p must be None or in [0, 1), got {min_p!r}")
+    sampled = [do_sample] * B if isinstance(do_sample, numbers.Real) else list(do_sample)
+    if len(sampled) != B:
+        return None         # generate_text_batch reports the wrong length of do_sample
+    if not any(s and (k > 0 or p < 1.0 or m > 0.0) for s, k, p, m in zip(sampled, ks, ps, ms)):
+        return None
+    return [int(k) for k in ks], [float(p) for p in ps], [float(m) for m in ms]
+
+
 def _capture_graph(launch: Callable[[], None], what: str) -> Optional[torch.cuda.CUDAGraph]:
     """Capture launch() as a CUDA graph and replay it once (capture does not execute the work). Capture is an
     optimisation and the eager launch sequence is the same work: on failure, warn, synchronise and return None."""
@@ -977,7 +1012,8 @@ class Bagel:
                             do_sample: Union[bool, Sequence[bool]] = False,
                             temperature: Union[float, Sequence[float]] = 1.0, end_token_id: Optional[int] = None,
                             seeds: Optional[Sequence[int]] = None,
-                            keys: Optional[Sequence[int]] = None) -> List[torch.Tensor]:
+                            keys: Optional[Sequence[int]] = None, top_k=None, top_p=None,
+                            min_p=None) -> List[torch.Tensor]:
         """Decode a batch of independent requests (same inputs as generate_text). Returns one LongTensor per request on
         the model's device: its tokens from the start token up to, not including, its own `end_token_id`, at most
         `max_length` of them. A finished request's token, sequence length and position freeze while the others go on.
@@ -991,12 +1027,21 @@ class Bagel:
 
         max_length, do_sample and temperature may each be one value per request instead of one for all. The step then
         picks every row with ops.sample_rows_mixed (greedy rows take argmax_rows' pick, sampled rows sample_rows' pick
-        at their own temperature) and stops each request at its own limit with ops.decode_advance_stop_limits."""
+        at their own temperature) and stops each request at its own limit with ops.decode_advance_stop_limits.
+
+        top_k (int, None or 0: off), top_p (in (0, 1], None or 1: off) and min_p (in [0, 1), None or 0: off), each one
+        value or one per request, truncate a sampled request's distribution as Hugging Face generate's warpers do, in
+        that order (greedy requests ignore them): the draw keeps the logits at or above the largest of the three
+        thresholds, computed on the device inside the step (ops.sample_rows_filtered; include/bagel_b200.h has the
+        exact definitions, ties at the top-k and top-p boundaries are kept). When no sampled request sets one, the step
+        runs exactly the launches it runs without them."""
         if self.dtype_mode == "B":
             raise NotImplementedError("generate_text_batch: the device-resident decode loop is implemented for dtype_mode='A'")
         dev = self.device
         B = int(torch.as_tensor(key_values_lens).numel())
-        per_request = not all(isinstance(x, numbers.Real) for x in (max_length, do_sample, temperature))
+        filters = _sampling_filters(B, do_sample, top_k, top_p, min_p)
+        per_request = filters is not None or not all(isinstance(x, numbers.Real)
+                                                     for x in (max_length, do_sample, temperature))
         if per_request:
             max_length, do_sample, temperature = (
                 [x] * B if isinstance(x, numbers.Real) else list(x) for x in (max_length, do_sample, temperature))
@@ -1036,10 +1081,16 @@ class Bagel:
             inv_t = torch.from_numpy(np.array([np.float32(1.0) / np.float32(t) if s else np.float32(0.0)
                                                for s, t in zip(do_sample, temperature)], dtype=np.float32)).to(dev)
             lim_dev = torch.tensor([max(n, 1) for n in limits], dtype=torch.int32, device=dev)
+            if filters is not None:
+                k_dev = torch.tensor(filters[0], dtype=torch.int32, device=dev)
+                p_dev, m_dev = (torch.tensor(f, dtype=torch.float32, device=dev) for f in filters[1:])
 
             def step_fn():
                 body()
-                ops.sample_rows_mixed(logits, inv_t, keys, step_dev, nxt)
+                if filters is None:
+                    ops.sample_rows_mixed(logits, inv_t, keys, step_dev, nxt)
+                else:
+                    ops.sample_rows_filtered(logits, inv_t, k_dev, p_dev, m_dev, keys, step_dev, nxt)
                 ops.decode_advance_stop_limits(d["seq_len"], d["pos"], d["tokens"], d["tokens32"], nxt, history,
                                                step_dev, finished, unfinished, end_token_id, lim_dev, self.HISTORY_PAD)
         else:
@@ -1086,7 +1137,7 @@ class Bagel:
     @torch.no_grad()
     def chat_batch(self, tokenizer, new_token_ids, image_transform, requests: Sequence[Tuple[Sequence[Any], str]],
                    max_length: int, do_sample: bool = False, temperature: float = 1.0,
-                   seeds: Optional[Sequence[int]] = None) -> List[str]:
+                   seeds: Optional[Sequence[int]] = None, top_k=None, top_p=None, min_p=None) -> List[str]:
         """`chat` for a batch of independent requests, each `(images, prompt)` with any number of images (zero
         included); returns one answer per request, cut at its own <|im_end|> as `chat` does.
 
@@ -1094,9 +1145,10 @@ class Bagel:
         images before r, never to later ones or to other requests. One SigLIP call covers every image of every
         request; then one LM prefill per image round r holds the r-th image of every request that has one (the others
         take part with no query tokens and their cached rows carried unchanged); then one prefill of all prompts and
-        one `generate_text_batch`."""
+        one `generate_text_batch` (top_k, top_p and min_p as there, one value or one per request)."""
         if self.dtype_mode == "B":
             raise NotImplementedError("chat_batch: the SigLIP prefill and the decode loop are implemented for dtype_mode='A'")
+        _sampling_filters(len(requests), do_sample, top_k, top_p, min_p, "chat_batch")   # refuse them before any prefill
         images = [list(imgs) for imgs, _ in requests]
         R = len(requests)
         newlens, new_rope = [0] * R, [0] * R
@@ -1124,7 +1176,8 @@ class Bagel:
         generation_input = self.prepare_start_tokens(newlens, new_rope, new_token_ids)
         answers = self.generate_text_batch(
             past_key_values=past_key_values, max_length=max_length, do_sample=do_sample, temperature=temperature,
-            end_token_id=new_token_ids["eos_token_id"], seeds=seeds, **generation_input)
+            end_token_id=new_token_ids["eos_token_id"], seeds=seeds, top_k=top_k, top_p=top_p, min_p=min_p,
+            **generation_input)
         return [tokenizer.decode(t).split("<|im_end|>")[0].split("<|im_start|>")[1] for t in answers]
 
     # ------------------------------------------------------------------------------------------

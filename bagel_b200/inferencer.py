@@ -16,6 +16,7 @@ from typing import Any, Dict, List, Optional, Sequence, Union
 
 import torch
 
+from .bagel import _sampling_filters
 from .qwen2_navit import NaiveCache, gather_requests
 
 VLM_THINK_SYSTEM_PROMPT = '''You should first think about the reasoning process in the mind and then provide the user with the answer. 
@@ -301,11 +302,13 @@ class InterleaveInferencer:
     # high word of the Philox key of call_batch's sampled text (the low word is the request's seed): a fixed stream
     # id, so a request's draws do not depend on its position in the batch
     TEXT_KEY_STREAM = 0x74657874
+    # optional truncation of a request's sampled thought or answer (Bagel.generate_text_batch); absent or None: off
+    TEXT_FILTERS = ("top_k", "top_p", "min_p")
 
     def _call_batch_requests(self, requests: Sequence[Dict[str, Any]]) -> List[Dict[str, Any]]:
         """call_batch's requests with their defaults filled in; refuses unknown keys, TaylorSeer and inputs that are
         neither a string nor an image."""
-        allowed = ("text", "image", "seed", "enable_taylorseer", *self.CALL_BATCH_DEFAULTS)
+        allowed = ("text", "image", "seed", "enable_taylorseer", *self.TEXT_FILTERS, *self.CALL_BATCH_DEFAULTS)
         unknown = [k for r in requests for k in r if k not in allowed]
         if unknown:
             raise ValueError(f"call_batch: unknown request keys {sorted(set(unknown))}")
@@ -313,6 +316,7 @@ class InterleaveInferencer:
             raise NotImplementedError("call_batch: TaylorSeer is not implemented for batched requests; use "
                                       "inferencer(..., enable_taylorseer=True) per request")
         for r in requests:
+            _sampling_filters(1, True, *(r.get(f) for f in self.TEXT_FILTERS), who="call_batch")
             if r.get("text") is not None and not isinstance(r["text"], str):
                 raise ValueError(f"call_batch: text must be a string, got {type(r['text'])}")
             if r.get("image") is not None and not _is_image(r["image"]):
@@ -329,8 +333,9 @@ class InterleaveInferencer:
         __call__; a request with neither gets {"image": None, "text": None}), `think`, `understanding_output`,
         `max_think_token_n`, `do_sample`, `text_temperature`, the image settings of gen_image_batch (`cfg_text_scale`,
         `cfg_img_scale`, `cfg_interval`, `cfg_renorm_min`, `cfg_renorm_type`, `image_shapes`) with the defaults of
-        interleave_inference, and `seed` (None: drawn from torch.default_generator). `enable_taylorseer=True` is
-        refused; num_timesteps and timestep_shift are shared.
+        interleave_inference, `top_k` / `top_p` / `min_p` (truncated sampling of its sampled thought or answer, see
+        Bagel.generate_text_batch; off when absent or None) and `seed` (None: drawn from torch.default_generator).
+        `enable_taylorseer=True` is refused; num_timesteps and timestep_shift are shared.
 
         Request q with seed s gets what `torch.manual_seed(s); inferencer(image=..., text=..., **its settings)` gives it
         alone: greedy text (do_sample=False) the same tokens up to bf16 ties; an image the same image whenever the
@@ -396,7 +401,8 @@ class InterleaveInferencer:
                 do_sample=[bool(reqs[q]["do_sample"]) for q in dec],
                 temperature=[float(reqs[q]["text_temperature"]) for q in dec],
                 end_token_id=self.new_token_ids["eos_token_id"],
-                keys=[(seeds[q] & 0xFFFFFFFF) | (self.TEXT_KEY_STREAM << 32) for q in dec], **gi)
+                keys=[(seeds[q] & 0xFFFFFFFF) | (self.TEXT_KEY_STREAM << 32) for q in dec],
+                **{f: [reqs[q].get(f) for q in dec] for f in self.TEXT_FILTERS}, **gi)
             for q, t in zip(dec, toks):
                 results[q]["text"] = self.tokenizer.decode(t.tolist()).split("<|im_end|>")[0].split("<|im_start|>")[1]
         main = text_round(main, only(sched["thought"], lambda q: results[q]["text"]))

@@ -522,6 +522,24 @@ def sample_rows_mixed(logits: torch.Tensor, inv_temperature: torch.Tensor, keys:
     _cabi.check(rc, "bagel_sample_rows_mixed_bf16")
 
 
+def sample_rows_filtered(logits: torch.Tensor, inv_temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
+                         min_p: torch.Tensor, keys: torch.Tensor, step_dev: torch.Tensor, tokens: torch.Tensor,
+                         tokens32: Optional[torch.Tensor] = None):
+    """sample_rows_mixed with per-row top-k (int32, <= 0 off), top-p (fp32, >= 1 off) and min-p (fp32, <= 0 off) for
+    the sampled rows, all [B] on the device; see include/bagel_b200.h."""
+    _req(logits, torch.bfloat16, "logits"); _req(inv_temperature, torch.float32, "inv_temperature")
+    _req(top_k, torch.int32, "top_k"); _req(top_p, torch.float32, "top_p"); _req(min_p, torch.float32, "min_p")
+    _req(keys, torch.int64, "keys"); _req(step_dev, torch.int32, "step_dev"); _req(tokens, torch.int64, "tokens")
+    _opt(tokens32, torch.int32, "tokens32")
+    B, V = logits.shape
+    assert inv_temperature.numel() == top_k.numel() == top_p.numel() == min_p.numel() == B
+    assert keys.numel() == tokens.numel() == B and (tokens32 is None or tokens32.numel() == B)
+    rc = _cabi.lib().bagel_sample_rows_filtered_bf16(
+        _ptr(logits), logits.stride(0), B, V, _ptr(inv_temperature), _ptr(top_k), _ptr(top_p), _ptr(min_p), _ptr(keys),
+        _ptr(step_dev), _ptr(tokens), _ptr(tokens32), _stream())
+    _cabi.check(rc, "bagel_sample_rows_filtered_bf16")
+
+
 def decode_advance_stop_limits(seq_len, pos, tokens, tokens32, next_tokens, history, step_dev, finished, unfinished,
                                end_token_id: Optional[int], max_length: torch.Tensor, pad: int):
     """decode_advance_stop with a limit per request (max_length int32 [B] on the device; history [rows, B]); see

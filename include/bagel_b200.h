@@ -277,6 +277,23 @@ int bagel_decode_advance_stop_limits(int* seq_len, long long* pos, long long* to
                                      int* unfinished, long long end_token_id, const int* max_length, int history_rows,
                                      long long pad, int B, void* stream);
 
+/* Truncated sampling (top-k, top-p, min-p, in the meaning of Hugging Face generate), one launch, graph-replayable:
+ *   bagel_sample_rows_filtered_bf16: bagel_sample_rows_mixed_bf16 with per-row filters for the sampled rows (greedy
+ *     rows ignore them). With l_j the row's bf16 logits, inv_t = inv_temperature[b] and l_max its largest finite logit:
+ *       top_k[b] > 0 keeps l_j >= the top_k[b]-th largest finite value counted with multiplicity (ties at the boundary
+ *         are kept; every finite logit when there are fewer);
+ *       top_p[b] < 1 keeps, among the logits top-k keeps, l_j >= the largest value v whose mass sum_{l_j >= v} e_j
+ *         reaches top_p[b] * sum e_j, e_j = exp((l_j - l_max) * inv_t) (ties decided by value, not by sort order);
+ *       min_p[b] > 0 keeps (l_j - l_max) * inv_t >= log(min_p[b]), in fp32.
+ *     Together they keep l_j >= one floor per row, and the row draws exactly as bagel_sample_rows_bf16 does (same key,
+ *     counter and word per logit) among those logits only. With every filter off (top_k <= 0, top_p >= 1, min_p <= 0)
+ *     a row's pick is bagel_sample_rows_mixed_bf16's, bit for bit. The mass is summed exactly in fixed point (each
+ *     fp32 e_j rounded to a multiple of 2^-40), so the pick does not depend on the batch or on launch order. NaN and
+ *     -inf are never kept; an all-NaN row yields token 0. B <= 1024, V <= 262144; tokens32 may be NULL. */
+int bagel_sample_rows_filtered_bf16(const void* logits, long long ld, int B, int V, const float* inv_temperature,
+                                    const int* top_k, const float* top_p, const float* min_p, const long long* keys,
+                                    const int* step_dev, long long* tokens, int* tokens32, void* stream);
+
 /* TaylorSeer step cache (reference modeling/cache_utils/taylorseer.py, enabled by generate_image(enable_taylorseer=True),
  * modeling/bagel/bagel.py:678-684; decoder-layer hooks modeling/bagel/qwen2_navit.py:773-777, 824-829).
  * factors: bf16 planes [order][rows][H], plane_stride elements apart, of the last decoder layer's output.
