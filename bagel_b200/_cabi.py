@@ -39,6 +39,7 @@ SIGNATURES = {
     "bagel_sample_rows_mixed_bf16": (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bagel_decode_advance_stop_limits": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp, _i, _ll, _i, _vp]),
     "bagel_sample_rows_filtered_bf16": (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bagel_apply_penalties_bf16": (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "bagel_rmsnorm_bf16": (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _ll, _i, _i, _f, _vp]),
     "bagel_layernorm_bf16": (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _f, _vp]),
     "bagel_rope_table": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),

@@ -15,6 +15,7 @@ What is different underneath (GPU-first, not a port):
 """
 from __future__ import annotations
 
+import math
 import numbers
 import warnings
 from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
@@ -209,6 +210,41 @@ def _sampling_filters(B: int, do_sample, top_k, top_p, min_p,
     if not any(s and (k > 0 or p < 1.0 or m > 0.0) for s, k, p, m in zip(sampled, ks, ps, ms)):
         return None
     return [int(k) for k in ks], [float(p) for p in ps], [float(m) for m in ms]
+
+
+def _penalties(B: int, repetition_penalty, presence_penalty, frequency_penalty,
+               who: str = "generate_text_batch") -> Optional[Tuple[List[float], List[float], List[float]]]:
+    """generate_text_batch's repetition_penalty (finite, > 0; None or 1: off), presence_penalty and frequency_penalty
+    (finite, in [-2, 2]; None or 0: off), each None, one value, or one per request, checked: per-request lists
+    (repetition, frequency, presence) for ops.apply_penalties, or None when every request has all three off."""
+    def expand(name, x):
+        if x is None or isinstance(x, numbers.Real):
+            return [x] * B
+        x = list(x)
+        if len(x) != B:
+            raise ValueError(f"{who}: {name} has {len(x)} entries for {B} requests")
+        return x
+
+    def real(v):
+        return isinstance(v, numbers.Real) and not isinstance(v, bool) and math.isfinite(v)
+
+    def positive_f32(r):         # the device divides by the fp32 value: it must be neither 0 nor inf
+        with np.errstate(over="ignore"):
+            return real(r) and r > 0.0 and 0.0 < np.float32(r) < np.inf
+
+    rs = [1.0 if r is None else r for r in expand("repetition_penalty", repetition_penalty)]
+    ps = [0.0 if p is None else p for p in expand("presence_penalty", presence_penalty)]
+    fs = [0.0 if f is None else f for f in expand("frequency_penalty", frequency_penalty)]
+    if not all(positive_f32(r) for r in rs):
+        raise ValueError(f"{who}: repetition_penalty must be None or finite and > 0, got {repetition_penalty!r}")
+    for name, xs, x in (("presence_penalty", ps, presence_penalty), ("frequency_penalty", fs, frequency_penalty)):
+        if not all(real(v) and -2.0 <= v <= 2.0 for v in xs):
+            raise ValueError(f"{who}: {name} must be None or in [-2, 2], got {x!r}")
+    # the device compares the fp32 values with the off values, so a value that rounds to one is off too
+    rs, fs, ps = ([float(np.float32(v)) for v in xs] for xs in (rs, fs, ps))
+    if all(r == 1.0 and f == 0.0 and p == 0.0 for r, f, p in zip(rs, fs, ps)):
+        return None
+    return rs, fs, ps
 
 
 def _capture_graph(launch: Callable[[], None], what: str) -> Optional[torch.cuda.CUDAGraph]:
@@ -1013,7 +1049,8 @@ class Bagel:
                             temperature: Union[float, Sequence[float]] = 1.0, end_token_id: Optional[int] = None,
                             seeds: Optional[Sequence[int]] = None,
                             keys: Optional[Sequence[int]] = None, top_k=None, top_p=None,
-                            min_p=None) -> List[torch.Tensor]:
+                            min_p=None, repetition_penalty=None, presence_penalty=None,
+                            frequency_penalty=None) -> List[torch.Tensor]:
         """Decode a batch of independent requests (same inputs as generate_text). Returns one LongTensor per request on
         the model's device: its tokens from the start token up to, not including, its own `end_token_id`, at most
         `max_length` of them. A finished request's token, sequence length and position freeze while the others go on.
@@ -1034,14 +1071,25 @@ class Bagel:
         that order (greedy requests ignore them): the draw keeps the logits at or above the largest of the three
         thresholds, computed on the device inside the step (ops.sample_rows_filtered; include/bagel_b200.h has the
         exact definitions, ties at the top-k and top-p boundaries are kept). When no sampled request sets one, the step
-        runs exactly the launches it runs without them."""
+        runs exactly the launches it runs without them.
+
+        repetition_penalty (finite, > 0; None or 1: off), presence_penalty and frequency_penalty (finite, in [-2, 2];
+        None or 0: off), each one value or one per request, penalise the tokens the request has generated in this call,
+        greedy and sampled requests alike, before temperature and the filters (Hugging Face's order: processors, then
+        warpers). With c_t the number of times token t was emitted so far (the start token and the prompt do not count),
+        each logit with c_t > 0 becomes bf16(((l < 0 ? l * rp : l / rp) - fp * c_t) - pp) in fp32, one rounding per
+        operation (ops.apply_penalties; include/bagel_b200.h). The repetition penalty is Hugging Face's
+        RepetitionPenaltyLogitsProcessor with prompt_ignore_length = the prompt's length, up to the final bf16 rounding;
+        presence and frequency are the OpenAI / vLLM penalties. The state costs 8 bytes per request per step of
+        max_length. When every request has all three off, the step runs exactly the launches it runs without them."""
         if self.dtype_mode == "B":
             raise NotImplementedError("generate_text_batch: the device-resident decode loop is implemented for dtype_mode='A'")
         dev = self.device
         B = int(torch.as_tensor(key_values_lens).numel())
         filters = _sampling_filters(B, do_sample, top_k, top_p, min_p)
-        per_request = filters is not None or not all(isinstance(x, numbers.Real)
-                                                     for x in (max_length, do_sample, temperature))
+        penalties = _penalties(B, repetition_penalty, presence_penalty, frequency_penalty)
+        per_request = filters is not None or penalties is not None or not all(
+            isinstance(x, numbers.Real) for x in (max_length, do_sample, temperature))
         if per_request:
             max_length, do_sample, temperature = (
                 [x] * B if isinstance(x, numbers.Real) else list(x) for x in (max_length, do_sample, temperature))
@@ -1084,9 +1132,14 @@ class Bagel:
             if filters is not None:
                 k_dev = torch.tensor(filters[0], dtype=torch.int32, device=dev)
                 p_dev, m_dev = (torch.tensor(f, dtype=torch.float32, device=dev) for f in filters[1:])
+            if penalties is not None:
+                rep_dev, freq_dev, pres_dev = (torch.tensor(x, dtype=torch.float32, device=dev) for x in penalties)
+                seen = ops.penalty_state(B, steps_max, dev)
 
             def step_fn():
                 body()
+                if penalties is not None:
+                    ops.apply_penalties(logits, rep_dev, freq_dev, pres_dev, d["tokens"], finished, step_dev, seen)
                 if filters is None:
                     ops.sample_rows_mixed(logits, inv_t, keys, step_dev, nxt)
                 else:
@@ -1137,7 +1190,8 @@ class Bagel:
     @torch.no_grad()
     def chat_batch(self, tokenizer, new_token_ids, image_transform, requests: Sequence[Tuple[Sequence[Any], str]],
                    max_length: int, do_sample: bool = False, temperature: float = 1.0,
-                   seeds: Optional[Sequence[int]] = None, top_k=None, top_p=None, min_p=None) -> List[str]:
+                   seeds: Optional[Sequence[int]] = None, top_k=None, top_p=None, min_p=None,
+                   repetition_penalty=None, presence_penalty=None, frequency_penalty=None) -> List[str]:
         """`chat` for a batch of independent requests, each `(images, prompt)` with any number of images (zero
         included); returns one answer per request, cut at its own <|im_end|> as `chat` does.
 
@@ -1145,10 +1199,14 @@ class Bagel:
         images before r, never to later ones or to other requests. One SigLIP call covers every image of every
         request; then one LM prefill per image round r holds the r-th image of every request that has one (the others
         take part with no query tokens and their cached rows carried unchanged); then one prefill of all prompts and
-        one `generate_text_batch` (top_k, top_p and min_p as there, one value or one per request)."""
+        one `generate_text_batch` (top_k, top_p, min_p, repetition_penalty, presence_penalty and frequency_penalty as
+        there, one value or one per request; the penalties count the answer's tokens only, not the images or the
+        prompt)."""
         if self.dtype_mode == "B":
             raise NotImplementedError("chat_batch: the SigLIP prefill and the decode loop are implemented for dtype_mode='A'")
-        _sampling_filters(len(requests), do_sample, top_k, top_p, min_p, "chat_batch")   # refuse them before any prefill
+        # refuse bad settings before any prefill
+        _sampling_filters(len(requests), do_sample, top_k, top_p, min_p, "chat_batch")
+        _penalties(len(requests), repetition_penalty, presence_penalty, frequency_penalty, "chat_batch")
         images = [list(imgs) for imgs, _ in requests]
         R = len(requests)
         newlens, new_rope = [0] * R, [0] * R
@@ -1177,7 +1235,8 @@ class Bagel:
         answers = self.generate_text_batch(
             past_key_values=past_key_values, max_length=max_length, do_sample=do_sample, temperature=temperature,
             end_token_id=new_token_ids["eos_token_id"], seeds=seeds, top_k=top_k, top_p=top_p, min_p=min_p,
-            **generation_input)
+            repetition_penalty=repetition_penalty, presence_penalty=presence_penalty,
+            frequency_penalty=frequency_penalty, **generation_input)
         return [tokenizer.decode(t).split("<|im_end|>")[0].split("<|im_start|>")[1] for t in answers]
 
     # ------------------------------------------------------------------------------------------

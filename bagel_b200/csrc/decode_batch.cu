@@ -439,6 +439,57 @@ sample_rows_filtered_kernel(const __nv_bfloat16* __restrict__ logits, long long 
   pick_row<true, true>(logits, ld, V, inv_t, keys, step_dev, tokens, tokens32, lfloor);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Repetition, frequency and presence penalties on the tokens a request has generated (see include/bagel_b200.h). The
+// state of row b is seen[b] = {n, tok[cap], cnt[cap]}: the n distinct tokens fed so far (step >= 1, while unfinished)
+// and how often each was fed, in order of first appearance. A step adds the token fed at it (tokens[b], chosen at the
+// previous step) with one thread, then rewrites each distinct token's logit once from the row it reads: O(n) work, no
+// atomics, and nothing depends on the order in which threads run.
+// ---------------------------------------------------------------------------------------------
+constexpr int kPenaltyThreads = 256;
+
+__global__ void __launch_bounds__(kPenaltyThreads)
+apply_penalties_kernel(__nv_bfloat16* __restrict__ logits, long long ld, int V, const float* __restrict__ repetition,
+                       const float* __restrict__ frequency, const float* __restrict__ presence,
+                       const long long* __restrict__ tokens, const int* __restrict__ finished,
+                       const int* __restrict__ step_dev, int* __restrict__ seen, int cap) {
+  const int b = blockIdx.x;
+  const float rp = repetition[b], fp = frequency[b], pp = presence[b];
+  if (rp == 1.0f && fp == 0.0f && pp == 0.0f) return;     // penalties off: the row is not touched
+  int* st = seen + (long long)b * (1 + 2 * (long long)cap);
+  int* tok = st + 1;
+  int* cnt = tok + cap;
+  __shared__ int s_hit;
+  int n = st[0];
+  const long long t = tokens[b];
+  if (step_dev[0] >= 1 && !finished[b] && t >= 0 && t < V) {
+    if (threadIdx.x == 0) s_hit = -1;
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += kPenaltyThreads)
+      if (tok[i] == static_cast<int>(t)) s_hit = i;         // the list is distinct: at most one thread writes
+    __syncthreads();
+    const int hit = s_hit;
+    if (hit < 0 && n < cap) {
+      if (threadIdx.x == 0) { tok[n] = static_cast<int>(t); cnt[n] = 1; st[0] = n + 1; }
+      ++n;
+    } else if (hit >= 0 && threadIdx.x == 0) {
+      cnt[hit] += 1;
+    }
+    __syncthreads();
+  }
+  __nv_bfloat16* row = logits + (long long)b * ld;
+  for (int i = threadIdx.x; i < n; i += kPenaltyThreads) {
+    const int j = tok[i];
+    const float l = __bfloat162float(row[j]);
+    if (isnan(l)) continue;                                   // NaN keeps its bits
+    // one rounding per operation, in this order (the intrinsics are never contracted into an FMA)
+    float r = l < 0.0f ? __fmul_rn(l, rp) : __fdiv_rn(l, rp);
+    r = __fsub_rn(r, __fmul_rn(fp, static_cast<float>(cnt[i])));
+    r = __fsub_rn(r, pp);
+    row[j] = __float2bfloat16_rn(r);
+  }
+}
+
 // Per-request stopping. A live request records its current token, then either takes next[b] (seq_len / pos advance)
 // or finishes: next[b] is the end token, or its history is full. A finished request keeps its token, seq_len and pos,
 // so the step it keeps running rewrites its own last K/V slot with the same values and never leaves its slab.
@@ -577,6 +628,24 @@ extern "C" int bagel_sample_rows_filtered_bf16(const void* logits, long long ld,
   sample_rows_filtered_kernel<<<B, kSampleThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(logits), ld, V, inv_temperature, top_k, top_p, min_p, keys, step_dev, tokens,
       tokens32);
+  COUNT_LAUNCH();
+  BAGEL_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int bagel_apply_penalties_bf16(void* logits, long long ld, int B, int V, const float* repetition,
+                                          const float* frequency, const float* presence, const long long* tokens,
+                                          const int* finished, const int* step_dev, int* seen, int capacity,
+                                          void* stream) {
+  if (B <= 0 || V <= 0) return 0;
+  if (ld < V) return set_error(BAGEL_ERR_SHAPE, "bagel_apply_penalties_bf16: ld must be >= V");
+  if (capacity <= 0) return set_error(BAGEL_ERR_SHAPE, "bagel_apply_penalties_bf16: capacity must be > 0");
+  if (logits == nullptr || repetition == nullptr || frequency == nullptr || presence == nullptr || tokens == nullptr ||
+      finished == nullptr || step_dev == nullptr || seen == nullptr)
+    return set_error(BAGEL_ERR_ARG, "bagel_apply_penalties_bf16: every pointer is required");
+  apply_penalties_kernel<<<B, kPenaltyThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<__nv_bfloat16*>(logits), ld, V, repetition, frequency, presence, tokens, finished, step_dev, seen,
+      capacity);
   COUNT_LAUNCH();
   BAGEL_CUDA_CHECK(cudaGetLastError());
   return 0;

@@ -16,7 +16,7 @@ from typing import Any, Dict, List, Optional, Sequence, Union
 
 import torch
 
-from .bagel import _sampling_filters
+from .bagel import _penalties, _sampling_filters
 from .qwen2_navit import NaiveCache, gather_requests
 
 VLM_THINK_SYSTEM_PROMPT = '''You should first think about the reasoning process in the mind and then provide the user with the answer. 
@@ -304,11 +304,15 @@ class InterleaveInferencer:
     TEXT_KEY_STREAM = 0x74657874
     # optional truncation of a request's sampled thought or answer (Bagel.generate_text_batch); absent or None: off
     TEXT_FILTERS = ("top_k", "top_p", "min_p")
+    # optional penalties on the tokens a request's thought or answer has generated (Bagel.generate_text_batch);
+    # absent or None: off
+    TEXT_PENALTIES = ("repetition_penalty", "presence_penalty", "frequency_penalty")
 
     def _call_batch_requests(self, requests: Sequence[Dict[str, Any]]) -> List[Dict[str, Any]]:
         """call_batch's requests with their defaults filled in; refuses unknown keys, TaylorSeer and inputs that are
         neither a string nor an image."""
-        allowed = ("text", "image", "seed", "enable_taylorseer", *self.TEXT_FILTERS, *self.CALL_BATCH_DEFAULTS)
+        allowed = ("text", "image", "seed", "enable_taylorseer", *self.TEXT_FILTERS, *self.TEXT_PENALTIES,
+                   *self.CALL_BATCH_DEFAULTS)
         unknown = [k for r in requests for k in r if k not in allowed]
         if unknown:
             raise ValueError(f"call_batch: unknown request keys {sorted(set(unknown))}")
@@ -317,6 +321,7 @@ class InterleaveInferencer:
                                       "inferencer(..., enable_taylorseer=True) per request")
         for r in requests:
             _sampling_filters(1, True, *(r.get(f) for f in self.TEXT_FILTERS), who="call_batch")
+            _penalties(1, *(r.get(f) for f in self.TEXT_PENALTIES), who="call_batch")
             if r.get("text") is not None and not isinstance(r["text"], str):
                 raise ValueError(f"call_batch: text must be a string, got {type(r['text'])}")
             if r.get("image") is not None and not _is_image(r["image"]):
@@ -334,7 +339,10 @@ class InterleaveInferencer:
         `max_think_token_n`, `do_sample`, `text_temperature`, the image settings of gen_image_batch (`cfg_text_scale`,
         `cfg_img_scale`, `cfg_interval`, `cfg_renorm_min`, `cfg_renorm_type`, `image_shapes`) with the defaults of
         interleave_inference, `top_k` / `top_p` / `min_p` (truncated sampling of its sampled thought or answer, see
-        Bagel.generate_text_batch; off when absent or None) and `seed` (None: drawn from torch.default_generator).
+        Bagel.generate_text_batch; off when absent or None), `repetition_penalty` / `presence_penalty` /
+        `frequency_penalty` (penalties on the tokens its thought or answer has generated, greedy or sampled, see
+        Bagel.generate_text_batch; off when absent or None; __call__ has no penalties) and `seed` (None: drawn from
+        torch.default_generator).
         `enable_taylorseer=True` is refused; num_timesteps and timestep_shift are shared.
 
         Request q with seed s gets what `torch.manual_seed(s); inferencer(image=..., text=..., **its settings)` gives it
@@ -402,7 +410,7 @@ class InterleaveInferencer:
                 temperature=[float(reqs[q]["text_temperature"]) for q in dec],
                 end_token_id=self.new_token_ids["eos_token_id"],
                 keys=[(seeds[q] & 0xFFFFFFFF) | (self.TEXT_KEY_STREAM << 32) for q in dec],
-                **{f: [reqs[q].get(f) for q in dec] for f in self.TEXT_FILTERS}, **gi)
+                **{f: [reqs[q].get(f) for q in dec] for f in self.TEXT_FILTERS + self.TEXT_PENALTIES}, **gi)
             for q, t in zip(dec, toks):
                 results[q]["text"] = self.tokenizer.decode(t.tolist()).split("<|im_end|>")[0].split("<|im_start|>")[1]
         main = text_round(main, only(sched["thought"], lambda q: results[q]["text"]))

@@ -540,6 +540,30 @@ def sample_rows_filtered(logits: torch.Tensor, inv_temperature: torch.Tensor, to
     _cabi.check(rc, "bagel_sample_rows_filtered_bf16")
 
 
+def penalty_state(B: int, capacity: int, device) -> torch.Tensor:
+    """Zeroed state of apply_penalties for B requests and at most `capacity` decode steps: int32 [B, 1 + 2 * capacity]
+    (per request: the number of distinct generated tokens, the tokens, their counts)."""
+    return torch.zeros((B, 1 + 2 * capacity), dtype=torch.int32, device=device)
+
+
+def apply_penalties(logits: torch.Tensor, repetition: torch.Tensor, frequency: torch.Tensor, presence: torch.Tensor,
+                    tokens: torch.Tensor, finished: torch.Tensor, step_dev: torch.Tensor, seen: torch.Tensor):
+    """In place: the repetition (fp32, 1 off), frequency and presence (fp32, 0 off) penalties of each row [B] on the
+    logits of the tokens it has generated, after adding this step's fed token (tokens[b], unless step_dev[0] == 0 or
+    finished[b]) to its state `seen` (penalty_state); see include/bagel_b200.h."""
+    _req(logits, torch.bfloat16, "logits"); _req(repetition, torch.float32, "repetition")
+    _req(frequency, torch.float32, "frequency"); _req(presence, torch.float32, "presence")
+    _req(tokens, torch.int64, "tokens"); _req(finished, torch.int32, "finished"); _req(step_dev, torch.int32, "step_dev")
+    _req(seen, torch.int32, "seen")
+    B, V = logits.shape
+    assert repetition.numel() == frequency.numel() == presence.numel() == tokens.numel() == finished.numel() == B
+    assert seen.dim() == 2 and seen.is_contiguous() and seen.shape[0] == B and seen.shape[1] % 2 == 1
+    rc = _cabi.lib().bagel_apply_penalties_bf16(
+        _ptr(logits), logits.stride(0), B, V, _ptr(repetition), _ptr(frequency), _ptr(presence), _ptr(tokens),
+        _ptr(finished), _ptr(step_dev), _ptr(seen), seen.shape[1] // 2, _stream())
+    _cabi.check(rc, "bagel_apply_penalties_bf16")
+
+
 def decode_advance_stop_limits(seq_len, pos, tokens, tokens32, next_tokens, history, step_dev, finished, unfinished,
                                end_token_id: Optional[int], max_length: torch.Tensor, pad: int):
     """decode_advance_stop with a limit per request (max_length int32 [B] on the device; history [rows, B]); see

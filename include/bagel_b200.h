@@ -294,6 +294,26 @@ int bagel_sample_rows_filtered_bf16(const void* logits, long long ld, int B, int
                                     const int* top_k, const float* top_p, const float* min_p, const long long* keys,
                                     const int* step_dev, long long* tokens, int* tokens32, void* stream);
 
+/* Generation penalties (Hugging Face RepetitionPenaltyLogitsProcessor with prompt_ignore_length = the prompt's length,
+ * and the OpenAI / vLLM presence and frequency penalties), one launch, graph-replayable; runs after the lm_head GEMM
+ * and before the step's pick, and modifies logits in place:
+ *   bagel_apply_penalties_bf16: with step = step_dev[0], G_b the tokens fed to request b at steps 1..step (the start
+ *     token fed at step 0 is not in it, and a finished request adds nothing) and c_t the number of times t occurs in
+ *     G_b, every logit l_t of row b with c_t > 0 is replaced, in fp32 with one rounding per operation (no FMA):
+ *       r = l_t < 0 ? l_t * repetition[b] : l_t / repetition[b];  r = r - frequency[b] * c_t;  r = r - presence[b];
+ *       l_t = bf16_rne(r).
+ *     Logits of tokens not in G_b, NaN logits (bits kept) and every logit of a row with repetition[b] == 1,
+ *     frequency[b] == 0 and presence[b] == 0 are untouched; -inf stays -inf for finite penalties. The launch at step
+ *     first adds tokens[b] to G_b when step >= 1, finished[b] == 0 and 0 <= tokens[b] < V, so it must run once per
+ *     step, before bagel_decode_advance_stop(_limits) of that step.
+ *     seen is int32 [B][1 + 2 * capacity], zeroed before step 0 and owned by the kernel: the number of distinct tokens
+ *     of G_b, then those tokens in order of first appearance, then their counts. capacity >= the number of steps
+ *     (tokens beyond capacity distinct ones are not counted). Work per row is O(distinct tokens); no atomics, so a
+ *     row's result depends only on its own logits, settings and tokens. */
+int bagel_apply_penalties_bf16(void* logits, long long ld, int B, int V, const float* repetition,
+                               const float* frequency, const float* presence, const long long* tokens,
+                               const int* finished, const int* step_dev, int* seen, int capacity, void* stream);
+
 /* TaylorSeer step cache (reference modeling/cache_utils/taylorseer.py, enabled by generate_image(enable_taylorseer=True),
  * modeling/bagel/bagel.py:678-684; decoder-layer hooks modeling/bagel/qwen2_navit.py:773-777, 824-829).
  * factors: bf16 planes [order][rows][H], plane_stride elements apart, of the last decoder layer's output.

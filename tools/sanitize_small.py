@@ -65,6 +65,10 @@ i32 = lambda *v: torch.tensor(v, dtype=torch.int32, device=dev)
 ops.sample_rows_filtered(lg2, torch.tensor([0.0, 2.0, 1.5, 1.0], device=dev), i32(3, 0, 40, 5),
                          torch.tensor([0.5, 0.9, 0.7, 1.0], device=dev), torch.tensor([0.0, 0.0, 0.1, 0.2], device=dev),
                          torch.arange(4, device=dev), sd, tk2, torch.empty(4, dtype=torch.int32, device=dev))
+# penalties: one row off, a finished row, unaligned ld; the step adds each live row's fed token
+ops.apply_penalties(lg2, torch.tensor([1.0, 1.05, 0.8, 1.0], device=dev), torch.tensor([0.0, 0.5, -1.0, 0.0], device=dev),
+                    torch.tensor([0.0, 0.2, 0.0, 1.5], device=dev), tk2, i32(0, 0, 1, 0), i32(1),
+                    ops.penalty_state(4, 3, dev))
 ops.decode_advance_stop_limits(i32(3, 4, 5, 6), torch.arange(4, device=dev), tk2.clone(), tk2.to(torch.int32), tk2,
                                torch.zeros(3, 4, dtype=torch.int64, device=dev), sd, i32(0, 0, 1, 0), i32(4), 5,
                                i32(1, 3, 2, 5), -1)
