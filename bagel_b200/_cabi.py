@@ -31,6 +31,8 @@ SIGNATURES = {
                                       _vp, _vp, _ll, _vp, _i, _i, _f, _i, _vp]),
     "bagel_attn_varlen_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f,
                                    _ll, _ll, _ll, _ll, _vp, _vp]),
+    "bagel_attn_decode_shared_bf16": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f,
+                                           _ll, _ll, _ll, _ll, _vp]),
     "bagel_decode_prepare": (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
     "bagel_argmax_rows_bf16": (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp]),
     "bagel_decode_advance": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp]),

@@ -247,6 +247,36 @@ def _penalties(B: int, repetition_penalty, presence_penalty, frequency_penalty,
     return rs, fs, ps
 
 
+def _num_samples(R: int, num_samples, who: str = "generate_text_batch") -> Optional[List[int]]:
+    """num_samples (None, one int >= 1, or one per request), checked: one count per request, or None."""
+    if num_samples is None:
+        return None
+    ns = [num_samples] * R if isinstance(num_samples, numbers.Number) else list(num_samples)
+    if len(ns) != R:
+        raise ValueError(f"{who}: num_samples has {len(ns)} entries for {R} requests")
+    if not all(isinstance(n, numbers.Integral) and not isinstance(n, bool) and n >= 1 for n in ns):
+        raise ValueError(f"{who}: num_samples must be an int >= 1 or one per request, got {num_samples!r}")
+    return [int(n) for n in ns]
+
+
+def _sample_keys(seeds: Sequence[int], ns: Sequence[int]) -> List[int]:
+    """Philox key of sample j of request i among R: (seeds[i] & 0xFFFFFFFF) | ((i + R * j) << 32), request-major. With
+    every n_i = 1 this is request i's key (seed, i); no two samples share a key."""
+    R = len(ns)
+    return [(int(sd) & 0xFFFFFFFF) | ((i + R * j) << 32) for i, (sd, n) in enumerate(zip(seeds, ns)) for j in range(n)]
+
+
+def _per_sample(x, ns: List[int]):
+    """A per-request setting as generate_text_batch takes it (None, one value, or one per request) for the decode rows
+    of num_samples ns: one value stays, a per-request list repeats each entry n_i times."""
+    if x is None or isinstance(x, numbers.Number):
+        return x
+    x = list(x)
+    if len(x) != len(ns):
+        return x            # the row-level check reports the wrong length
+    return [v for v, n in zip(x, ns) for _ in range(n)]
+
+
 def _capture_graph(launch: Callable[[], None], what: str) -> Optional[torch.cuda.CUDAGraph]:
     """Capture launch() as a CUDA graph and replay it once (capture does not execute the work). Capture is an
     optimisation and the eager launch sequence is the same work: on failure, warn, synchronise and return None."""
@@ -941,24 +971,34 @@ class Bagel:
     # text decode
     # ------------------------------------------------------------------------------------------
     def _decode_state(self, past_key_values: Optional[NaiveCache], key_values_lens, packed_start_tokens,
-                      packed_query_position_ids, max_length: int) -> Dict[str, Any]:
+                      packed_query_position_ids, max_length: int,
+                      num_samples: Optional[Sequence[int]] = None) -> Dict[str, Any]:
         """Device state of a decode of `max_length` steps and its step body (embedding gather -> `run_layers` on a
         decode `ForwardPlan` -> final norm -> lm_head into `logits`). Every buffer the body touches is fixed, so the
-        body is graph-replayable."""
+        body is graph-replayable. num_samples (one int >= 1 per request): request i continues as that many decode rows,
+        request-major, over one copy of its context (ForwardPlan.decode_shared); the per-row state starts from the
+        request's start token, position and context length."""
         dev = self.device
         lm = self.language_model.model
         cfg = lm.config
         L, w = cfg.num_hidden_layers, cfg.num_key_value_heads * cfg.head_dim
         kv = torch.as_tensor(key_values_lens).to("cpu", torch.int64)
+        if num_samples is None:
+            plan = ForwardPlan.decode(lm, kv, max_length)
+        else:
+            plan = ForwardPlan.decode_shared(lm, kv, num_samples, max_length)
+            rows = torch.repeat_interleave(torch.arange(kv.numel()), torch.as_tensor(list(num_samples)))
+            kv = kv[rows]
+            packed_start_tokens = torch.as_tensor(packed_start_tokens).cpu()[rows]
+            packed_query_position_ids = torch.as_tensor(packed_query_position_ids).cpu()[rows]
         B = int(kv.numel())
-        plan = ForwardPlan.decode(lm, kv, max_length)
         # zero-filled, not torch.empty: attention multiplies the masked probabilities (exactly 0) with whatever sits in the
         # spare rows of a slab — 0 x NaN/Inf garbage would poison the output (the attention kernel fetches whole 128-key
         # blocks by TMA; only the single-query d=128 kernel clamps its loads to the rows in use)
         kbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
         vbuf = torch.zeros((L, plan.total_kv, w), dtype=BF16, device=dev)
         if past_key_values is not None and past_key_values.key_cache[0] is not None and plan.n_ctx:
-            lm.place_context(past_key_values, plan.ctx_rows, kbuf, vbuf)
+            lm.place_context(past_key_values, plan.ctx_rows, kbuf, vbuf, src_rows=plan.ctx_src)
         st: Dict[str, Any] = {"B": B}
         st["seq_len"] = seq_len = kv.to(dev, torch.int32)
         st["pos"] = pos = torch.as_tensor(packed_query_position_ids).to(dev, torch.int64).clone()
@@ -1050,7 +1090,7 @@ class Bagel:
                             seeds: Optional[Sequence[int]] = None,
                             keys: Optional[Sequence[int]] = None, top_k=None, top_p=None,
                             min_p=None, repetition_penalty=None, presence_penalty=None,
-                            frequency_penalty=None) -> List[torch.Tensor]:
+                            frequency_penalty=None, num_samples=None) -> Union[List[torch.Tensor], List[List[torch.Tensor]]]:
         """Decode a batch of independent requests (same inputs as generate_text). Returns one LongTensor per request on
         the model's device: its tokens from the start token up to, not including, its own `end_token_id`, at most
         `max_length` of them. A finished request's token, sequence length and position freeze while the others go on.
@@ -1081,11 +1121,42 @@ class Bagel:
         operation (ops.apply_penalties; include/bagel_b200.h). The repetition penalty is Hugging Face's
         RepetitionPenaltyLogitsProcessor with prompt_ignore_length = the prompt's length, up to the final bf16 rounding;
         presence and frequency are the OpenAI / vLLM penalties. The state costs 8 bytes per request per step of
-        max_length. When every request has all three off, the step runs exactly the launches it runs without them."""
+        max_length. When every request has all three off, the step runs exactly the launches it runs without them.
+
+        num_samples (an int >= 1, or one per request) asks for n_i samples of request i: the call then returns one list
+        of n_i token tensors per request. Sample j of request i is a decode row of its own with the request's settings
+        and its own stop, penalty state and Philox key (seed_i & 0xFFFFFFFF) | ((i + R * j) << 32), R requests, so
+        sample 0 keeps the key the request has without num_samples; `keys` then holds one key per sample, sum(n_i)
+        of them, request-major. When ForwardPlan.decode_shared's rule picks the shared layout, the context is placed in
+        the KV slab once per request and the decode attention reads it once per 4 samples (ops.attn_decode_shared);
+        otherwise each sample gets a copy of it. With every n_i = 1 the step is exactly the step without num_samples."""
         if self.dtype_mode == "B":
             raise NotImplementedError("generate_text_batch: the device-resident decode loop is implemented for dtype_mode='A'")
         dev = self.device
         B = int(torch.as_tensor(key_values_lens).numel())
+        ns = _num_samples(B, num_samples)
+        if ns is not None:
+            # request-level checks, then every per-request setting becomes a per-row one
+            _sampling_filters(B, do_sample, top_k, top_p, min_p)
+            _penalties(B, repetition_penalty, presence_penalty, frequency_penalty)
+            for name, x in (("max_length", max_length), ("do_sample", do_sample), ("temperature", temperature)):
+                if not isinstance(x, numbers.Number) and len(list(x)) != B:
+                    raise ValueError(f"generate_text_batch: {name} has {len(list(x))} entries for {B} requests")
+            if keys is None:
+                if seeds is None:
+                    base = int(torch.randint(0, 2 ** 32, (1,), dtype=torch.int64))
+                    seeds = [base] * B
+                elif len(seeds) != B:
+                    raise ValueError(f"generate_text_batch: {len(seeds)} seeds for {B} requests")
+                keys = _sample_keys(seeds, ns)
+            elif len(keys) != sum(ns):
+                raise ValueError(f"generate_text_batch: {len(keys)} keys for {sum(ns)} samples")
+            max_length, do_sample, temperature, top_k, top_p, min_p, repetition_penalty, presence_penalty, \
+                frequency_penalty = (_per_sample(x, ns) for x in (
+                    max_length, do_sample, temperature, top_k, top_p, min_p, repetition_penalty, presence_penalty,
+                    frequency_penalty))
+            B = sum(ns)
+        plan_samples = ns if ns is not None and max(ns) > 1 else None    # all ones: the step without num_samples
         filters = _sampling_filters(B, do_sample, top_k, top_p, min_p)
         penalties = _penalties(B, repetition_penalty, presence_penalty, frequency_penalty)
         per_request = filters is not None or penalties is not None or not all(
@@ -1105,18 +1176,18 @@ class Bagel:
                 raise ValueError("generate_text_batch: do_sample=True needs a finite temperature > 0")
             steps_max = max_length
         if steps_max <= 0:
-            return [torch.zeros(0, dtype=torch.int64, device=dev) for _ in range(B)]
+            return self._by_request([torch.zeros(0, dtype=torch.int64, device=dev) for _ in range(B)], ns)
         if keys is None:
             if seeds is None:
                 base = int(torch.randint(0, 2 ** 32, (1,), dtype=torch.int64))
                 seeds = [base] * B
             elif len(seeds) != B:
                 raise ValueError(f"generate_text_batch: {len(seeds)} seeds for {B} requests")
-            keys = [(int(sd) & 0xFFFFFFFF) | (i << 32) for i, sd in enumerate(seeds)]
+            keys = _sample_keys(seeds, [1] * B)
         elif len(keys) != B:
             raise ValueError(f"generate_text_batch: {len(keys)} keys for {B} requests")
         d = self._decode_state(past_key_values, key_values_lens, packed_start_tokens, packed_query_position_ids,
-                               steps_max)
+                               steps_max, plan_samples)
         body, logits, history, step_dev = d["body"], d["logits"], d["history"], d["step_dev"]
         keys = torch.from_numpy(np.array([int(k) & 0xFFFFFFFFFFFFFFFF for k in keys], dtype=np.uint64).view(np.int64)).to(dev)
         nxt = torch.empty(B, dtype=torch.int64, device=dev)
@@ -1185,13 +1256,22 @@ class Bagel:
         lens = (hist != self.HISTORY_PAD).sum(0).tolist()
         if per_request:
             lens = [min(n, lim) for n, lim in zip(lens, limits)]
-        return [hist[:n, i].clone() for i, n in enumerate(lens)]
+        return self._by_request([hist[:n, i].clone() for i, n in enumerate(lens)], ns)
+
+    @staticmethod
+    def _by_request(outs: List[Any], ns: Optional[List[int]]):
+        """Per-row results as generate_text_batch returns them: as they are, or one list of n_i per request."""
+        if ns is None:
+            return outs
+        first = np.cumsum([0] + ns)
+        return [outs[a:b] for a, b in zip(first[:-1], first[1:])]
 
     @torch.no_grad()
     def chat_batch(self, tokenizer, new_token_ids, image_transform, requests: Sequence[Tuple[Sequence[Any], str]],
                    max_length: int, do_sample: bool = False, temperature: float = 1.0,
                    seeds: Optional[Sequence[int]] = None, top_k=None, top_p=None, min_p=None,
-                   repetition_penalty=None, presence_penalty=None, frequency_penalty=None) -> List[str]:
+                   repetition_penalty=None, presence_penalty=None, frequency_penalty=None,
+                   num_samples=None) -> Union[List[str], List[List[str]]]:
         """`chat` for a batch of independent requests, each `(images, prompt)` with any number of images (zero
         included); returns one answer per request, cut at its own <|im_end|> as `chat` does.
 
@@ -1201,12 +1281,16 @@ class Bagel:
         take part with no query tokens and their cached rows carried unchanged); then one prefill of all prompts and
         one `generate_text_batch` (top_k, top_p, min_p, repetition_penalty, presence_penalty and frequency_penalty as
         there, one value or one per request; the penalties count the answer's tokens only, not the images or the
-        prompt)."""
+        prompt).
+
+        num_samples (an int >= 1, or one per request) returns n_i answers per request, as generate_text_batch's
+        num_samples: each request's context is built once, whatever its n_i."""
         if self.dtype_mode == "B":
             raise NotImplementedError("chat_batch: the SigLIP prefill and the decode loop are implemented for dtype_mode='A'")
         # refuse bad settings before any prefill
         _sampling_filters(len(requests), do_sample, top_k, top_p, min_p, "chat_batch")
         _penalties(len(requests), repetition_penalty, presence_penalty, frequency_penalty, "chat_batch")
+        ns = _num_samples(len(requests), num_samples, "chat_batch")
         images = [list(imgs) for imgs, _ in requests]
         R = len(requests)
         newlens, new_rope = [0] * R, [0] * R
@@ -1236,8 +1320,13 @@ class Bagel:
             past_key_values=past_key_values, max_length=max_length, do_sample=do_sample, temperature=temperature,
             end_token_id=new_token_ids["eos_token_id"], seeds=seeds, top_k=top_k, top_p=top_p, min_p=min_p,
             repetition_penalty=repetition_penalty, presence_penalty=presence_penalty,
-            frequency_penalty=frequency_penalty, **generation_input)
-        return [tokenizer.decode(t).split("<|im_end|>")[0].split("<|im_start|>")[1] for t in answers]
+            frequency_penalty=frequency_penalty, num_samples=ns, **generation_input)
+
+        def text(t):
+            return tokenizer.decode(t).split("<|im_end|>")[0].split("<|im_start|>")[1]
+        if ns is None:
+            return [text(t) for t in answers]
+        return [[text(t) for t in ts] for ts in answers]
 
     # ------------------------------------------------------------------------------------------
     # training-mode forward (losses only, no backward): reference Bagel.forward, bagel.py:101-229

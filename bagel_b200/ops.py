@@ -220,6 +220,38 @@ def attn_varlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens_q:
     return out
 
 
+def attn_decode_shared_supported(Hq: int, Hk: int, head_dim: int) -> bool:
+    """The shapes bagel_attn_decode_shared_bf16 takes: head_dim 128, Hq / Hk in {1, 2, 4, 7, 8}."""
+    return head_dim == 128 and Hk > 0 and Hq % Hk == 0 and Hq // Hk in (1, 2, 4, 7, 8)
+
+
+def attn_decode_shared(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_rows: torch.Tensor,
+                       prefix_begin: torch.Tensor, prefix_len: torch.Tensor, suffix_begin: torch.Tensor,
+                       seqused_k: torch.Tensor, max_group_rows: int, max_seqlen_k: int,
+                       softmax_scale: Optional[float] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One query row per decode row against its group's shared prefix keys, then its own suffix keys: q [rows,Hq,D],
+    k/v [Sk,Hk,D] bf16, int32 device index arrays; see include/bagel_b200.h."""
+    _req(q, torch.bfloat16, "q"); _req(k, torch.bfloat16, "k"); _req(v, torch.bfloat16, "v")
+    for t, nm in ((cu_rows, "cu_rows"), (prefix_begin, "prefix_begin"), (prefix_len, "prefix_len"),
+                  (suffix_begin, "suffix_begin"), (seqused_k, "seqused_k")):
+        _req(t, torch.int32, nm)
+    rows, Hq, D = q.shape
+    _, Hk, _ = k.shape
+    assert q.stride(1) == D and k.stride(1) == D and v.stride(1) == D, "heads must be contiguous"
+    groups = cu_rows.numel() - 1
+    assert prefix_begin.numel() == prefix_len.numel() == groups and suffix_begin.numel() == seqused_k.numel() == rows
+    if out is None:
+        out = torch.empty((rows, Hq, D), dtype=torch.bfloat16, device=q.device)
+    if softmax_scale is None:
+        softmax_scale = D ** -0.5
+    rc = _cabi.lib().bagel_attn_decode_shared_bf16(
+        _ptr(q), _ptr(k), _ptr(v), _ptr(out), _ptr(cu_rows), _ptr(prefix_begin), _ptr(prefix_len), _ptr(suffix_begin),
+        _ptr(seqused_k), groups, rows, int(max_group_rows), Hq, Hk, D, int(max_seqlen_k), float(softmax_scale),
+        q.stride(0), k.stride(0), v.stride(0), out.stride(0), _stream())
+    _cabi.check(rc, "bagel_attn_decode_shared_bf16")
+    return out
+
+
 def rmsnorm(x: torch.Tensor, w0: torch.Tensor, w1: Optional[torch.Tensor] = None,
             expert: Optional[torch.Tensor] = None, eps: float = 1e-6, out: Optional[torch.Tensor] = None):
     _req(x, torch.bfloat16, "x"); _req(w0, torch.bfloat16, "w0")

@@ -127,12 +127,20 @@ class _Layer:
         self.gen: Optional[_ExpertWeights] = None
 
 
+# decode_shared() lays a batch out with a shared context prefix when some request has at least SHARED_MIN_SAMPLES
+# samples and at least SHARED_MIN_CTX_PER_SAMPLE context tokens per sample
+SHARED_MIN_SAMPLES = 5
+SHARED_MIN_CTX_PER_SAMPLE = 64
+
+
 class ForwardPlan:
     """Everything about one packed LM call that does not depend on the hidden states: int32 index maps on the
     device, cu_seqlens, RoPE tables, which QKV path runs. Built once per call (or once per denoising run, or once
     per decode) so the layer loop is pure kernel launches with no host<->device synchronisation (the reference
     syncs >= 2x per layer, :585-586). The constructor plans a packed prefill / denoising call; `decode()` plans
     the one-token-per-sample step of text generation."""
+    shared: Optional["SharedPrefix"] = None     # set by decode_shared(): attention over a shared context prefix
+    ctx_src: Optional[torch.Tensor] = None      # cache row of each ctx_rows entry (None: the cache rows in order)
 
     def __init__(self, lm: "Qwen2Model", query_lens, position_ids, packed_query_indexes, key_values_lens,
                  packed_key_value_indexes, is_causal: bool, mode: str, packed_vae_token_indexes=None,
@@ -214,6 +222,58 @@ class ForwardPlan:
         p.expert = p.text_rows = None
         p.fuse_qkv = D == 128 and B > 64   # B <= 64: weight-streaming skinny GEMM + norm/RoPE kernel
         return p
+
+    @classmethod
+    def decode_shared(cls, lm: "Qwen2Model", key_values_lens, num_samples, max_length: int) -> "ForwardPlan":
+        """`decode()` for num_samples[i] decode rows per request i (request-major), every row of request i continuing
+        its key_values_lens[i] context rows. Request i owns one slab region: its context rows, placed once (ctx_rows),
+        then one suffix of `max_length` rows per sample, so the slab has sum(ctx) + sum(n) * max_length rows and
+        attention runs ops.attn_decode_shared over `shared`. cu_k[r] = suffix_begin[r] - ctx_i is the base that
+        ops.decode_prepare adds seq_len[r] (= ctx_i + tokens so far) to: q_rows[r] is the row's next suffix row and
+        seqused_k[r] its key count, prefix included.
+        Batches where no request has n >= SHARED_MIN_SAMPLES samples and ctx >= SHARED_MIN_CTX_PER_SAMPLE * n context
+        rows, and shapes the shared kernel does not take (head_dim 64, other GQA groups), get `decode()` over each
+        request's context repeated per row instead, with ctx_src the cache row each placed row copies. On an H100 the
+        shared kernel measured slower than attn_decode on the replicated layout at up to 4 samples (one pass: a
+        quarter of the CTAs to stream the same prefix) and at 32 samples of a 797-token context, and faster at 8
+        samples of 797 and 8 or 32 samples of 3721 tokens (README)."""
+        cfg = lm.config
+        kv = torch.as_tensor(key_values_lens).to("cpu", torch.int64).reshape(-1)
+        ns = torch.as_tensor(num_samples).to("cpu", torch.int64).reshape(-1)
+        assert ns.numel() == kv.numel() and bool((ns >= 1).all()), "one num_samples >= 1 per request"
+        row_kv = torch.repeat_interleave(kv, ns)
+        pays = bool(((ns >= SHARED_MIN_SAMPLES) & (kv >= SHARED_MIN_CTX_PER_SAMPLE * ns)).any())
+        if not pays or not ops.attn_decode_shared_supported(cfg.num_attention_heads, cfg.num_key_value_heads,
+                                                            cfg.head_dim):
+            p = cls.decode(lm, row_kv, max_length)
+            p.ctx_src = _ranges(torch.repeat_interleave(torch.cumsum(kv, 0) - kv, ns), row_kv).to(lm.device, torch.int32)
+            return p
+        dev = lm.device
+        R, B = int(kv.numel()), int(ns.sum())
+        cap = kv + ns * max_length
+        begin = torch.cumsum(cap, 0) - cap
+        req = torch.repeat_interleave(torch.arange(R), ns)
+        first_row = torch.cumsum(ns, 0) - ns
+        suffix_begin = begin[req] + kv[req] + (torch.arange(B) - first_row[req]) * max_length
+        p = cls.decode(lm, row_kv, max_length)    # per-row state buffers, cos/sin, QKV path: as for B independent rows
+        p.n_ctx, p.total_kv = int(kv.sum()), int(cap.sum())
+        p.cu_k = torch.cat([suffix_begin - row_kv, torch.tensor([p.total_kv])]).to(dev, torch.int32)
+        p.ctx_rows = _ranges(begin, kv).to(dev, torch.int32)
+        z = torch.zeros(1, dtype=torch.int64)
+        p.shared = SharedPrefix(cu_rows=torch.cat([z, ns.cumsum(0)]).to(dev, torch.int32),
+                                prefix_begin=begin.to(dev, torch.int32), prefix_len=kv.to(dev, torch.int32),
+                                suffix_begin=suffix_begin.to(dev, torch.int32), max_group_rows=int(ns.max()))
+        return p
+
+
+@dataclass
+class SharedPrefix:
+    """Index arrays (int32, on the device) of ops.attn_decode_shared for a ForwardPlan.decode_shared plan."""
+    cu_rows: torch.Tensor
+    prefix_begin: torch.Tensor
+    prefix_len: torch.Tensor
+    suffix_begin: torch.Tensor
+    max_group_rows: int
 
 
 class Qwen2Model:
@@ -382,8 +442,15 @@ class Qwen2Model:
                 ops.qk_norm_rope(qkv, und.q_norm, und.k_norm, amain.q_norm if a_routed else None,
                                  amain.k_norm if a_routed else None, a_expert, plan.cos, plan.sin, q, kbuf[li], vbuf[li],
                                  plan.q_rows, Hq, Hk, D, eps, plan.fp32_flow)
-            ops.attn_varlen(q.view(n, Hq, D), kbuf[li].view(-1, Hk, D), vbuf[li].view(-1, Hk, D), plan.cu_q, plan.cu_k,
-                            plan.max_q, plan.max_k, plan.is_causal, out=att.view(n, Hq, D), seqused_k=plan.seqused_k)
+            if plan.shared is not None:
+                sh = plan.shared
+                ops.attn_decode_shared(q.view(n, Hq, D), kbuf[li].view(-1, Hk, D), vbuf[li].view(-1, Hk, D), sh.cu_rows,
+                                       sh.prefix_begin, sh.prefix_len, sh.suffix_begin, plan.seqused_k,
+                                       sh.max_group_rows, plan.max_k, out=att.view(n, Hq, D))
+            else:
+                ops.attn_varlen(q.view(n, Hq, D), kbuf[li].view(-1, Hk, D), vbuf[li].view(-1, Hk, D), plan.cu_q,
+                                plan.cu_k, plan.max_q, plan.max_k, plan.is_causal, out=att.view(n, Hq, D),
+                                seqused_k=plan.seqused_k)
             ops.gemm(att, amain.wo, resid=xa, epilogue=EPI_R, out=xb)
             if nta:
                 ops.copy_rows(att, at, src_rows=plan.text_rows)

@@ -124,6 +124,23 @@ int bagel_attn_varlen_fwd(const void* q, const void* k, const void* v, void* out
                           float softmax_scale, long long ld_q, long long ld_k, long long ld_v, long long ld_out,
                           const int* seqused_k, void* stream);
 
+/* Shared-prefix single-query attention (the decode step of several samples of one prompt): `groups` groups of decode
+ * rows, group g owning rows [cu_rows[g], cu_rows[g+1]) (consecutive, at most max_group_rows of them). Row r of group g
+ * attends with one softmax (fp32, scale softmax_scale) to the keys
+ *   [prefix_begin[g], prefix_begin[g] + prefix_len[g])  followed by  [suffix_begin[r], suffix_begin[r] + u_r),
+ *   u_r = max(seqused_k[r] - prefix_len[g], 0),
+ * of k/v [*, Hk, 128] bf16 (row strides ld_k, ld_v). q [rows, Hq, 128], out [rows, Hq, 128] bf16 (ld_q, ld_out), query
+ * row r at row r; a row with no key gets zeros. All index arrays are int32 DEVICE arrays (cu_rows [groups + 1],
+ * prefix_* [groups], suffix_begin / seqused_k [rows]); max_seqlen_k (host, <= 0 if unknown) bounds prefix_len + u_r
+ * and only tunes the key split. One prefix K/V tile read from HBM serves up to 4 rows of a group. Hq / Hk must be 1,
+ * 2, 4, 7 or 8 and head_dim 128 (BAGEL_ERR_SHAPE otherwise). The summation order depends only on a group's own
+ * lengths, with no atomics: the result of a row does not depend on the other groups or on launch order. */
+int bagel_attn_decode_shared_bf16(const void* q, const void* k, const void* v, void* out, const int* cu_rows,
+                                  const int* prefix_begin, const int* prefix_len, const int* suffix_begin,
+                                  const int* seqused_k, int groups, int rows, int max_group_rows, int num_heads_q,
+                                  int num_heads_k, int head_dim, int max_seqlen_k, float softmax_scale, long long ld_q,
+                                  long long ld_k, long long ld_v, long long ld_out, void* stream);
+
 /* y = bf16(w_e * bf16(x * rsqrt(mean(x^2) + eps))), e = expert[row] ? w1 : w0 (expert / w1 may be NULL).
  * Qwen2RMSNorm (modeling/qwen2/modeling_qwen2.py:54-59) with the MoT row routing of
  * modeling/bagel/qwen2_navit.py:781-787, 808-815, 1075-1082. x, y bf16 [N, H]. */
