@@ -207,6 +207,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const __nv_bfloat16* rrow = (EPI == EPI_RESID) ? p.resid + out_row * p.ldr + n0_tile : nullptr;
           const float* rrow32 = (EPI == EPI_RESID_F32) ? p.resid32 + out_row * p.ldr + n0_tile : nullptr;
           float* crow32 = (EPI == EPI_F32 || EPI == EPI_RESID_F32) ? p.C32 + out_row * p.ldc + n0_tile : nullptr;
+          // The row's residuals are all loaded before its first store: C may alias resid, so the compiler cannot move a
+          // load above an earlier store, and loads interleaved with the stores would be BN / 8 dependent round trips.
+          uint32_t rres[EPI == EPI_RESID ? BN / 8 : 1];
+          if constexpr (EPI == EPI_RESID) {
+#pragma unroll
+            for (int c = 0; c < BN / 8; ++c)
+              if (n0_tile + 8 * c + cq < p.N) rres[c] = *reinterpret_cast<const uint32_t*>(rrow + 8 * c + cq);
+          }
 #pragma unroll
           for (int c = 0; c < BN / 8; ++c) {
             const int n = 8 * c + cq;              // N % 8 == 0: a column pair is in or out together
@@ -218,7 +226,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               x1 += bf16_hi(bb);
             }
             if constexpr (EPI == EPI_RESID) {
-              const uint32_t rr = *reinterpret_cast<const uint32_t*>(rrow + n);
+              const uint32_t rr = rres[c];
               x0 = bf16_lo(rr) + bf16_round(x0);
               x1 = bf16_hi(rr) + bf16_round(x1);
             } else if constexpr (EPI == EPI_RESID_F32) {
